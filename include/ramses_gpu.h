@@ -211,7 +211,7 @@ int rgpu_comm_init(int nranks, int rank, const void* unique_id_128);
 
 /* ---- introspection (tests / bench) ---------------------------------------------- */
 typedef struct rgpu_level_info {
-  int dense;                 /* 1: dense-box fast path                             */
+  int dense;                 /* 1: dense-box fast path (AMR mode: the dense kernel sweeps the level) */
   int ncell_box[3];          /* box extent in cells                                */
   int own_lo[3], own_hi[3];  /* owned cell range                                   */
   int wrap[3];

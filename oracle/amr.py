@@ -21,12 +21,16 @@ class AmrRun:
     def __init__(self, ndim, levelmin, levelmax, bound_type, boxlen, nsubcycle, nexpand=1, ngridmax=2000,
                  riemann="hllc", slope_type=2, gamma=1.4, courant_factor=0.8, err_grad_d=-1.0, err_grad_u=-1.0,
                  err_grad_p=-1.0, interpol_type=1, interpol_var=0, regions=(), tout=(), nvector=32,
-                 floor_d=1e-10, floor_u=1e-10, floor_p=1e-10, bound_regions=None):
+                 floor_d=1e-10, floor_u=1e-10, floor_p=1e-10, bound_regions=None, coarse=(1, 1, 1)):
+        """coarse = (nx, ny, nz) domain coarse cells (orc_mesh_new_box); the mesh-adaptation driver itself is exercised with
+        one domain coarse cell, several are for trees fabricated elsewhere and loaded into son / father / nbor / lists."""
         self.ndim, self.levelmin, self.nlevelmax = ndim, levelmin, levelmax
         self.T, self.twondim = 1 << ndim, 2 * ndim
         L = self.L = orc.lib()
         L.orc_mesh_new.restype = C.POINTER(orc.MeshS)
         L.orc_mesh_new.argtypes = [C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int]
+        L.orc_mesh_new_box.restype = C.POINTER(orc.MeshS)
+        L.orc_mesh_new_box.argtypes = [C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.c_int]
         L.orc_mesh_set_list.argtypes = [C.POINTER(orc.MeshS), C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]
         L.orc_interpol_cell.argtypes = [C.POINTER(orc.Params), C.POINTER(orc.MeshS), C.c_int, C.c_int,
                                         C.POINTER(C.c_double), C.POINTER(C.c_double)]
@@ -34,7 +38,12 @@ class AmrRun:
         L.orc_set_interpol.argtypes = [C.c_int, C.c_int]
         L.orc_set_interpol(interpol_type, interpol_var)
         bt = (C.c_int * 6)(*bound_type)
-        self.mp = L.orc_mesh_new(ndim, bt, ngridmax, levelmax)
+        if tuple(coarse) == (1, 1, 1):
+            self.mp = L.orc_mesh_new(ndim, bt, ngridmax, levelmax)
+        else:
+            if any(coarse[d] != 1 for d in range(ndim, 3)) or min(coarse) < 1:
+                raise ValueError(f"coarse={coarse} does not fit ndim={ndim}")
+            self.mp = L.orc_mesh_new_box(ndim, (C.c_int * 3)(*coarse), bt, ngridmax, levelmax)
         self.m = self.mp.contents
         m = self.m
         self.ncoarse, self.ngridmax, self.ncell = m.ncoarse, m.ngridmax, m.ncell

@@ -70,6 +70,8 @@ def lib():
         mp = C.POINTER(MeshS)
         L.orc_mesh_build_uniform.restype = mp
         L.orc_mesh_build_uniform.argtypes = [C.c_int, C.c_int, ip, C.c_int, C.c_uint]
+        L.orc_mesh_build_box.restype = mp
+        L.orc_mesh_build_box.argtypes = [C.c_int, C.c_int, ip, ip, C.c_int, C.c_uint]
         L.orc_mesh_free.argtypes = [mp]
         L.orc_mesh_oct_pos.argtypes = [mp, C.c_int, C.c_int, ip]
         L.orc_get3cubefather.argtypes = [mp, C.c_int, C.c_int, ip, ip]
@@ -144,11 +146,17 @@ def make_params(ndim=3, nvar=None, nvector=32, slope_type=1, niter_riemann=10, r
 
 
 class Mesh:
-    """Fully refined oct tree (levels 1..levelmax) fabricated by the oracle's builder."""
+    """Fully refined oct tree (levels 1..levelmax) fabricated by the oracle's builder.  coarse = (nx, ny, nz): the domain
+    coarse cells (boundary coarse cells are added around them for every face with a boundary type)."""
 
-    def __init__(self, ndim, levelmax, bound_type=(0,) * 6, order=0, seed=1):
+    def __init__(self, ndim, levelmax, bound_type=(0,) * 6, order=0, seed=1, coarse=(1, 1, 1)):
         bt = (C.c_int * 6)(*bound_type)
-        self.ptr = lib().orc_mesh_build_uniform(ndim, levelmax, bt, order, seed)
+        if tuple(coarse) == (1, 1, 1):
+            self.ptr = lib().orc_mesh_build_uniform(ndim, levelmax, bt, order, seed)
+        else:
+            if any(coarse[d] != 1 for d in range(ndim, 3)) or min(coarse) < 1:
+                raise ValueError(f"coarse={coarse} does not fit ndim={ndim}")
+            self.ptr = lib().orc_mesh_build_box(ndim, levelmax, (C.c_int * 3)(*coarse), bt, order, seed)
         self.s = self.ptr.contents
         self.ndim, self.levelmax = ndim, levelmax
 
@@ -181,6 +189,15 @@ class Mesh:
         lib().orc_mesh_oct_pos(self.ptr, l, int(igrid), pos)
         return tuple(pos)
 
+    def coarse(self):
+        """domain coarse cells per axis (icoarse_max - icoarse_min + 1 etc.)"""
+        s = self.s
+        return (s.icoarse_max - s.icoarse_min + 1, s.jcoarse_max - s.jcoarse_min + 1, s.kcoarse_max - s.kcoarse_min + 1)
+
+    def extent(self, l):
+        """(nx, ny, nz) cells of the domain at level l (1 along the unused axes)"""
+        return tuple(self.coarse()[d] << l if d < self.ndim else 1 for d in range(3))
+
     def new_state(self, nvar):
         return np.zeros(nvar * self.s.ncell, dtype=np.float64)
 
@@ -195,8 +212,7 @@ class Mesh:
         pos = np.array([self.oct_pos(l, g) for g in ig], dtype=np.int64) if len(ig) < 5000 else self._pos_fast(l, ig)
         cmin = np.array([self.s.icoarse_min, self.s.jcoarse_min, self.s.kcoarse_min]) * (1 << (l - 1))
         pos = pos - cmin[None, :]
-        n = 1 << l
-        shape = [n if d < nd else 1 for d in range(3)]
+        shape = self.extent(l)
         out = np.zeros((nvar, shape[2], shape[1], shape[0]))
         uu = u.reshape(nvar, self.s.ncell)
         for ind in range(1 << nd):
@@ -209,6 +225,8 @@ class Mesh:
 
     def dense_to_level(self, dense, u, l, nvar):
         nd = self.ndim
+        ext = self.extent(l)
+        assert dense.shape[1:] == (ext[2], ext[1], ext[0]), (dense.shape, ext)
         ig = self.active(l).astype(np.int64)
         pos = self._pos_fast(l, ig)
         cmin = np.array([self.s.icoarse_min, self.s.jcoarse_min, self.s.kcoarse_min]) * (1 << (l - 1))

@@ -1114,11 +1114,20 @@ typedef struct { int pos[3]; int region; } octrec; /* region 0 domain, b>0 bound
 static unsigned lcg(unsigned* s) { *s = *s * 1664525u + 1013904223u; return *s >> 8; }
 
 orc_mesh* orc_mesh_build_uniform(int ndim, int levelmax, const int bt[6], int order, unsigned seed) {
+  static const int one[3] = {1, 1, 1};
+  return orc_mesh_build_box(ndim, levelmax, one, bt, order, seed);
+}
+
+/* the domain is ndom[0] x ndom[1] x ndom[2] coarse cells (nx, ny, nz of the namelist), every one refined to levelmax,
+ * plus one layer of boundary coarse cells on each face with a boundary type                                          */
+orc_mesh* orc_mesh_build_box(int ndim, int levelmax, const int ndom[3], const int bt[6], int order, unsigned seed) {
+  for (int d = 0; d < 3; d++)
+    if (ndom[d] < 1 || (d >= ndim && ndom[d] != 1)) { fprintf(stderr, "orc mesh: bad domain %d x %d x %d\n", ndom[0], ndom[1], ndom[2]); abort(); }
   orc_mesh* m = (orc_mesh*)calloc(1, sizeof(orc_mesh));
   m->ndim = ndim; m->nlevelmax = levelmax;
   const int twotondim = ipow2(ndim), twondim = 2 * ndim;
   /* coarse grid geometry: hydro/read_hydro_params.f90:316-350 */
-  int nn[3] = {1, 1, 1}, cmin[3] = {0, 0, 0}, cmax[3] = {0, 0, 0};
+  int nn[3] = {ndom[0], ndom[1], ndom[2]}, cmin[3] = {0, 0, 0}, cmax[3] = {ndom[0] - 1, ndom[1] - 1, ndom[2] - 1};
   m->nboundary = 0;
   int bface[ORC_MAXBOUND]; /* which face each boundary region covers: 2*d+s */
   for (int d = 0; d < ndim; d++)
@@ -1135,17 +1144,12 @@ orc_mesh* orc_mesh_build_uniform(int ndim, int levelmax, const int bt[6], int or
   m->jcoarse_min = cmin[1]; m->jcoarse_max = cmax[1];
   m->kcoarse_min = cmin[2]; m->kcoarse_max = cmax[2];
   m->ncoarse = nn[0] * nn[1] * nn[2];
-  /* count octs: level l has the domain octs 2^(ndim*(l-1)) plus one layer of boundary octs */
+  /* count octs: level l has the domain octs ndom[d] 2^(l-1) per axis plus one layer of boundary octs per boundary face */
   long total = 0;
   for (int l = 1; l <= levelmax; l++) {
-    long dom = 1, all = 1;
-    for (int d = 0; d < ndim; d++) {
-      long n = 1L << (l - 1);
-      dom *= n;
-      all *= n + (nn[d] - 1);
-    }
+    long all = 1;
+    for (int d = 0; d < ndim; d++) all *= ((long)ndom[d] << (l - 1)) + (nn[d] - ndom[d]);
     total += (l == 1) ? m->ncoarse : all;
-    (void)dom;
   }
   m->ngridmax = (int)total + 8;
   m->ncell = m->ncoarse + twotondim * m->ngridmax;
@@ -2079,9 +2083,16 @@ void orc_upload_fine(const orc_params* p, const orc_mesh* m, int ilevel, double*
 /* an empty mesh (coarse grid only) whose tree arrays the AMR driver (oracle/amr.py) fills in like
  * amr/refine_utils.f90 does; lists are pushed with orc_mesh_set_list                                 */
 orc_mesh* orc_mesh_new(int ndim, const int bt[6], int ngridmax, int nlevelmax) {
+  static const int one[3] = {1, 1, 1};
+  return orc_mesh_new_box(ndim, one, bt, ngridmax, nlevelmax);
+}
+/* the same on a domain of ndom[0] x ndom[1] x ndom[2] coarse cells (see orc_mesh_build_box) */
+orc_mesh* orc_mesh_new_box(int ndim, const int ndom[3], const int bt[6], int ngridmax, int nlevelmax) {
+  for (int d = 0; d < 3; d++)
+    if (ndom[d] < 1 || (d >= ndim && ndom[d] != 1)) { fprintf(stderr, "orc mesh: bad domain %d x %d x %d\n", ndom[0], ndom[1], ndom[2]); abort(); }
   orc_mesh* m = (orc_mesh*)calloc(1, sizeof(orc_mesh));
   m->ndim = ndim; m->nlevelmax = nlevelmax;
-  int nn[3] = {1, 1, 1}, cmin[3] = {0, 0, 0}, cmax[3] = {0, 0, 0};
+  int nn[3] = {ndom[0], ndom[1], ndom[2]}, cmin[3] = {0, 0, 0}, cmax[3] = {ndom[0] - 1, ndom[1] - 1, ndom[2] - 1};
   for (int d = 0; d < ndim; d++)
     for (int s2 = 0; s2 < 2; s2++)
       if (bt[2 * d + s2] > 0) {

@@ -93,6 +93,9 @@ void orc_cmpdt(const orc_params*, double* uu, const double* gg, double dx, doubl
  * cell position outermost: amr/refine_utils.f90 make_grid_fine order),
  * 1 = lattice row-major, 2 = pseudo-random permutation (seed).               */
 orc_mesh* orc_mesh_build_uniform(int ndim, int levelmax, const int bound_type[6], int order, unsigned seed);
+/* the same on a domain of ndom[0] x ndom[1] x ndom[2] coarse cells (nx, ny, nz of AMR_PARAMS; ndom[d] = 1 for d >= ndim),
+ * boundary coarse cells added around it as above; build_uniform is build_box with a single domain cell                */
+orc_mesh* orc_mesh_build_box(int ndim, int levelmax, const int ndom[3], const int bound_type[6], int order, unsigned seed);
 void      orc_mesh_free(orc_mesh*);
 /* integer position of every oct of a level in units of oct size (for tests)   */
 void orc_mesh_oct_pos(const orc_mesh*, int ilevel, int igrid, int pos[3]);
@@ -133,6 +136,7 @@ void orc_getnborfather(const orc_mesh*, int ind_cell, int ilevel, int* ind_fathe
 void orc_interpol_hydro(const orc_params*, const double* u1 /*[2*ndim+1][nvar]*/, double* u2 /*[2^ndim][nvar]*/);
 void orc_interpol_cell(const orc_params*, const orc_mesh*, int ind_cell, int ilevel, const double* uold, double* u2);
 orc_mesh* orc_mesh_new(int ndim, const int bound_type[6], int ngridmax, int nlevelmax);
+orc_mesh* orc_mesh_new_box(int ndim, const int ndom[3], const int bound_type[6], int ngridmax, int nlevelmax);
 void orc_mesh_set_list(orc_mesh*, int kind, int b, int ilevel, int n, const int* igrid);
 
 /* pressure_fix: caller-owned divu / enew cell arrays [ncell] (NULL = off) and beta_fix (amr_parameters.f90:167)      */

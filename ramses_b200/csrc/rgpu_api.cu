@@ -2372,8 +2372,17 @@ int rgpu_comm_init(int nranks, int rank, const void* unique_id_128) {
 
 int rgpu_get_level_info(int ilevel, rgpu_level_info* o) {
   if (G.init && G.amr && o && ilevel >= 1 && ilevel <= MAXLEVEL && G.alev[ilevel].bound) {
+    const AmrLevel& A = G.alev[ilevel];
     memset(o, 0, sizeof(*o));
-    o->nslot = G.alev[ilevel].nact; o->kernel_launches = G.alev[ilevel].launches; o->last_steps_ms = G.alev[ilevel].last_steps_ms;
+    o->nslot = A.nact; o->kernel_launches = A.launches; o->last_steps_ms = A.last_steps_ms;
+    if (A.dense_sweep) {   // the dense kernel's AMR variant sweeps the level (base box or refined patch): report its box
+      const DenseGeom& g = G.lev[ilevel].g;
+      o->dense = 1;
+      o->ncell_box[0] = g.ncx; o->ncell_box[1] = g.ncy; o->ncell_box[2] = g.ncz;
+      o->own_lo[0] = g.ox0; o->own_lo[1] = g.oy0; o->own_lo[2] = g.oz0;
+      o->own_hi[0] = g.ox1; o->own_hi[1] = g.oy1; o->own_hi[2] = g.oz1;
+      o->wrap[0] = g.wrapx; o->wrap[1] = g.wrapy; o->wrap[2] = g.wrapz;
+    }
     return RGPU_OK;
   }
   if (!G.init || ilevel < 1 || ilevel > MAXLEVEL || !G.lev[ilevel].bound || !o) return fail(RGPU_EINVAL, "level %d not bound", ilevel);

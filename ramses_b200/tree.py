@@ -223,25 +223,27 @@ def fill_state(a, ilevel, fn):
 def build_nested_tree(levelmin, levelmax, half_width=8, boxlen=1.0, nvar=None, mhd=False):
     """A statically refined 3-D periodic tree (single rank): levels 1..levelmin cover the box, every level
     levelmin < l <= levelmax refines the centred cube of (2*half_width)^3 cells of level l-1 (so each fine level holds
-    (2*half_width)^3 octs).  With half_width >= 2 every refined cell keeps its 3^3 neighbours at its own level, the
-    rule the reference enforces through smooth_fine / nexpand (amr/flag_utils.f90:117-188), and a fine oct's six
-    neighbouring father cells always exist.  Produces the arrays of amr/amr_commons.f90:68-79 like build_uniform_tree;
-    oct numbering is lattice order level by level."""
+    (2*half_width)^3 octs); half_width = (hx, hy, hz) refines a centred box of 2hx x 2hy x 2hz cells instead.  With
+    every half width >= 2 every refined cell keeps its 3^3 neighbours at its own level, the rule the reference enforces
+    through smooth_fine / nexpand (amr/flag_utils.f90:117-188), and a fine oct's six neighbouring father cells always
+    exist.  Produces the arrays of amr/amr_commons.f90:68-79 like build_uniform_tree; oct numbering is lattice order
+    level by level."""
     ndim, nx, ny, nz = 3, 1, 1, 1
     nvar = nvar or (8 if mhd else 5)
-    if half_width < 2:
+    hw = np.array(half_width if hasattr(half_width, "__len__") else (half_width,) * 3, dtype=np.int64)
+    if hw.shape != (3,) or hw.min() < 2:
         raise ValueError("half_width must be >= 2")
     pos = {}
     for l in range(1, levelmax + 1):
         n = 1 << (l - 1)                                  # octs per dimension if the level were full
         if l <= levelmin:
-            r = np.arange(n)
+            r = [np.arange(n)] * 3
         else:
             c = n // 2                                    # father cells at level l-1: n per dimension
-            if 2 * half_width > n:
-                raise ValueError("refined cube larger than the box")
-            r = np.arange(c - half_width, c + half_width)
-        gz, gy, gx = np.meshgrid(r, r, r, indexing="ij")
+            if (2 * hw > n).any():
+                raise ValueError("refined box larger than the box")
+            r = [np.arange(c - hw[d], c + hw[d]) for d in range(3)]
+        gz, gy, gx = np.meshgrid(r[2], r[1], r[0], indexing="ij")
         pos[l] = np.stack([gx.ravel(), gy.ravel(), gz.ravel()], axis=1).astype(np.int64)
     igrid0, nxt = {}, 1
     for l in range(1, levelmax + 1):
@@ -255,10 +257,10 @@ def build_nested_tree(levelmin, levelmax, half_width=8, boxlen=1.0, nvar=None, m
         p = np.mod(p, n)
         if l <= levelmin:
             return igrid0[l] + p[:, 0] + n * (p[:, 1] + n * p[:, 2])
-        c, h = n // 2, half_width
-        q = p - (c - h)
-        ok = np.all((q >= 0) & (q < 2 * h), axis=1)
-        return np.where(ok, igrid0[l] + q[:, 0] + 2 * h * (q[:, 1] + 2 * h * q[:, 2]), 0)
+        c = n // 2
+        q = p - (c - hw)[None, :]
+        ok = np.all((q >= 0) & (q < 2 * hw[None, :]), axis=1)
+        return np.where(ok, igrid0[l] + q[:, 0] + 2 * hw[0] * (q[:, 1] + 2 * hw[1] * q[:, 2]), 0)
 
     a = AmrCommons(ndim, nvar, ncoarse, ngridmax, nx, ny, nz, (0, 0), (0, 0), (0, 0), nlevelmax=levelmax, boxlen=boxlen, mhd=mhd)
     for l in range(1, levelmax + 1):

@@ -47,9 +47,10 @@ class Case:
     """One run set-up: oracle mesh + params + the Fortran-side arrays (AmrCommons)."""
 
     def __init__(self, ndim, level, riemann="hllc", slope_type=1, bound=(0,) * 6, order=0, seed=1, boxlen=1.0,
-                 gamma=1.4, courant_factor=0.8, niter_riemann=10, slope_theta=1.5, nvector=32, nvar=None):
+                 gamma=1.4, courant_factor=0.8, niter_riemann=10, slope_theta=1.5, nvector=32, nvar=None, coarse=(1, 1, 1)):
+        """coarse = (nx, ny, nz) domain coarse cells; dx = boxlen / nx / 2^level"""
         self.ndim, self.level, self.nvar = ndim, level, (nvar or ndim + 2)      # nvar > ndim+2: passive scalars
-        self.mesh = orc.Mesh(ndim, level, bound, order, seed)
+        self.mesh = orc.Mesh(ndim, level, bound, order, seed, coarse=coarse)
         self.p = orc.make_params(ndim=ndim, nvar=self.nvar, riemann=riemann, slope_type=slope_type, boxlen=boxlen, gamma=gamma,
                                  courant_factor=courant_factor, niter_riemann=niter_riemann, slope_theta=slope_theta,
                                  nvector=nvector)
@@ -166,6 +167,88 @@ def mhd_smooth_state(n, gamma=5.0 / 3.0, b0=(0.5, 0.3, 0.2), amp=0.1, periodic=(
     return u
 
 
+def mhd_box_state(ext, gamma=5.0 / 3.0, b0=(0.5, 0.3, 0.2), amp=0.1):
+    """mhd_smooth_state on a box of ext = (nx, ny, nz) cells of size h = 1/nx: one wave across the box per axis (different
+    periods per axis), divergence-free staggered field from an edge-centred vector potential that is periodic on the box.
+    Returns the dense conservative array [11][nz][ny][nx]."""
+    nx, ny, nz = ext
+    h = 1.0 / nx
+    k = [2 * np.pi / (e * h) for e in ext]
+    xc = [(np.arange(e) + 0.5) * h for e in ext]
+    xe = [np.arange(e) * h for e in ext]
+    Z, Y, X = np.meshgrid(xc[2], xc[1], xc[0], indexing="ij")
+    d = 1 + 0.2 * np.sin(k[0] * X) * np.cos(k[1] * Y) + 0.1 * np.sin(k[2] * Z + 0.7)
+    vel = [0.3 * np.sin(k[1] * Y), 0.2 * np.cos(k[2] * Z), 0.1 * np.sin(k[0] * X)]
+    P = 1 + 0.1 * np.cos(k[2] * Z) * np.sin(k[0] * X + k[1] * Y)
+    ze, ye, _ = np.meshgrid(xe[2], xe[1], xc[0], indexing="ij"); Ax = amp * np.sin(k[1] * ye) * np.cos(k[2] * ze)
+    ze, _, xe_ = np.meshgrid(xe[2], xc[1], xe[0], indexing="ij"); Ay = amp * np.sin(k[2] * ze + 1.0) * np.cos(k[0] * xe_)
+    _, ye, xe_ = np.meshgrid(xc[2], xe[1], xe[0], indexing="ij"); Az = amp * np.cos(k[0] * xe_) * np.sin(k[1] * ye + 0.3)
+    up = lambda a, ax: np.roll(a, -1, axis=ax)
+    bx = (up(Az, 1) - Az) / h - (up(Ay, 0) - Ay) / h + b0[0]
+    by = (up(Ax, 0) - Ax) / h - (up(Az, 2) - Az) / h + b0[1]
+    bz = (up(Ay, 2) - Ay) / h - (up(Ax, 1) - Ax) / h + b0[2]
+    u = np.zeros((11, nz, ny, nx))
+    u[0] = d
+    for c in range(3):
+        u[1 + c] = d * vel[c]
+    u[5], u[6], u[7] = bx, by, bz
+    u[8], u[9], u[10] = up(bx, 2), up(by, 1), up(bz, 0)
+    ekin = 0.5 * d * (vel[0] ** 2 + vel[1] ** 2 + vel[2] ** 2)
+    emag = 0.125 * ((u[5] + u[8]) ** 2 + (u[6] + u[9]) ** 2 + (u[7] + u[10]) ** 2)
+    u[4] = P / (gamma - 1.0) + ekin + emag
+    return u
+
+
+def box_state(ndim, ext, seed=3, gamma=1.4):
+    """a hydro state on a box of ext = (nx, ny, nz) cells (1 beyond ndim) of size h = 1/nx with no symmetry that could hide a
+    swapped axis: one wave across the box per axis, an off-centre Gaussian blob and seeded density jumps.  Periodic on the box
+    (the blob is small enough).  Returns the dense conservative array [ndim+2][nz][ny][nx]."""
+    h = 1.0 / ext[0]
+    L = [e * h for e in ext]
+    xs = [(np.arange(e) + 0.5) * h for e in ext]
+    Z, Y, X = np.meshgrid(xs[2], xs[1], xs[0], indexing="ij")
+    tw = 2 * np.pi
+    sx, sy, sz = tw * X / L[0], tw * Y / L[1], tw * Z / L[2]
+    r2 = ((X - 0.3 * L[0]) / (0.15 * L[0])) ** 2
+    if ndim > 1:
+        r2 = r2 + ((Y - 0.6 * L[1]) / (0.2 * L[1])) ** 2
+    if ndim > 2:
+        r2 = r2 + ((Z - 0.45 * L[2]) / (0.25 * L[2])) ** 2
+    blob = np.exp(-r2)
+    rho = 1 + 0.2 * np.sin(sx) * np.cos(sy) + 0.1 * np.sin(sz + 0.3) + 0.5 * blob
+    rho *= 1 + 0.3 * (np.random.default_rng(seed).standard_normal(rho.shape) > 1.3)
+    vel = [0.3 * np.sin(sy + 0.2) + 0.1 * np.cos(sz) + 0.1 * np.sin(sx), 0.25 * np.sin(sz) - 0.1 * np.sin(sx), 0.2 * np.sin(sx + 0.5)]
+    p = 1 + 0.1 * np.cos(sx + sy + sz) + 2.0 * blob
+    u = np.zeros((ndim + 2,) + rho.shape)
+    u[0] = rho
+    e = p / (gamma - 1)
+    for d in range(ndim):
+        u[1 + d] = rho * vel[d]
+        e = e + 0.5 * rho * vel[d] ** 2
+    u[ndim + 1] = e
+    return u
+
+
+def level_slots(mesh, l, u, nvar):
+    """The octs of level l of an oracle mesh (active and boundary octs) in the dense-box slot layout of the device (plan_level:
+    lattice order of the oct positions over the box spanned by them): returns uin [nvar][2^ndim][nslot] and the (igrid, slot)
+    of the active octs."""
+    nd = mesh.ndim
+    act = mesh.active(l).astype(np.int64)
+    ig = np.concatenate([act] + [mesh.bound(b, l).astype(np.int64) for b in range(mesh.s.nboundary)])
+    pos = mesh._pos_fast(l, ig)
+    lo = pos.min(axis=0)
+    no = pos.max(axis=0) - lo + 1
+    q = pos - lo
+    slot = q[:, 0] + no[0] * (q[:, 1] + no[1] * q[:, 2])
+    T = 1 << nd
+    U = u.reshape(nvar, mesh.s.ncell)
+    uin = np.zeros((nvar, T, int(no.prod())))
+    for ind in range(T):
+        uin[:, ind, slot] = U[:, mesh.s.ncoarse + ind * mesh.s.ngridmax + ig - 1]
+    return uin, act, slot[:len(act)]
+
+
 def mhd_tube_state(n, left, right, x0, boxlen, gamma):
     """Shock tube along x (mhd/condinit.f90 with two 'square' regions spanning y,z): left/right = (d,u,v,w,P,A,B,C)."""
     xc = (np.arange(n) + 0.5) * boxlen / n
@@ -190,9 +273,9 @@ class MhdCase:
     """MHD run set-up: oracle mesh + MHD params + the Fortran-side arrays (AmrCommons of an MHD build)."""
 
     def __init__(self, level, riemann="hlld", riemann2d="llf", slope_type=1, slope_mag_type=-1, bound=(0,) * 6, order=0, seed=1,
-                 boxlen=1.0, gamma=5.0 / 3.0, courant_factor=0.8, slope_theta=1.5):
+                 boxlen=1.0, gamma=5.0 / 3.0, courant_factor=0.8, slope_theta=1.5, coarse=(1, 1, 1)):
         self.ndim, self.level, self.nvar, self.nvs = 3, level, 8, 11
-        self.mesh = orc.Mesh(3, level, bound, order, seed)
+        self.mesh = orc.Mesh(3, level, bound, order, seed, coarse=coarse)
         self.p = orc.make_mhd_params(slope_type=slope_type, slope_mag_type=slope_mag_type, riemann=riemann, riemann2d=riemann2d,
                                      gamma=gamma, courant_factor=courant_factor, boxlen=boxlen, slope_theta=slope_theta)
         self.riemann, self.riemann2d, self.slope_type, self.slope_mag_type = riemann, riemann2d, slope_type, slope_mag_type

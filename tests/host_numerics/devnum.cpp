@@ -103,6 +103,27 @@ static void interpol_full_nd(int itype, int ivar, int n, const double* u1, doubl
     for (int t = 0; t < T; t++) for (int v = 0; v < NVX; v++) u2[(i * T + t) * NVX + v] = b[t][v];
   }
 }
+// dense-box geometry of an owned box of n[d] cells per axis, set the way plan_level (rgpu_api.cu) sets it: an axis without a
+// shell is periodic over the box, an axis with shell[d] != 0 carries one ghost oct (2 cells) on each side; n[d] = 1 beyond ndim
+static DenseGeom box_geom(int ndim, const int n[3], const int shell[3]) {
+  DenseGeom g;
+  std::memset(&g, 0, sizeof g);
+  int nc[3], o0[3], o1[3], wr[3];
+  for (int d = 0; d < 3; d++) {
+    const int sh = (d < ndim && shell[d]) ? 2 : 0;
+    nc[d] = d < ndim ? n[d] + 2 * sh : 1;
+    o0[d] = sh; o1[d] = d < ndim ? sh + n[d] : 1;
+    wr[d] = d < ndim && !shell[d];
+  }
+  g.ncx = nc[0]; g.ncy = nc[1]; g.ncz = nc[2];
+  g.nox = (nc[0] + 1) / 2; g.noy = (nc[1] + 1) / 2; g.noz = (nc[2] + 1) / 2;
+  g.ox0 = o0[0]; g.ox1 = o1[0]; g.oy0 = o0[1]; g.oy1 = o1[1]; g.oz0 = o0[2]; g.oz1 = o1[2];
+  g.wrapx = wr[0]; g.wrapy = wr[1]; g.wrapz = wr[2];
+  g.nslot = (long long)g.nox * g.noy * g.noz;
+  return g;
+}
+static const int k_no_shell[3] = {0, 0, 0};
+
 #pragma GCC visibility push(default)
 extern "C" {
 
@@ -560,19 +581,17 @@ void devnum_mhd_emf(int solver2d, int n, const double* qLL, const double* qRL, c
 
 // the six passes of the dense MHD sweep (mhd_dense.cuh) in the order of launch_mhd_sweep (mhd_inst_misc.cu) on a periodic cube
 // of N^3 cells: uin/uout in the device layout [11][8][nslot] (cell_offset of sweep_dense.cuh), N even
-void devnum_mhd_sweep(int N, int r1d, int r2d, int sl, const double* uin, double* uout, double dt, double dx, double gamma,
-                      double smallr, double smallc, int slope_type, int slope_mag_type) {
+// on a box of n[0] x n[1] x n[2] owned cells, each axis periodic or with a 2-cell ghost shell (box_geom)
+void devnum_mhd_sweep_box(const int* n, const int* shell, int r1d, int r2d, int sl, const double* uin, double* uout, double dt,
+                          double dx, double gamma, double smallr, double smallc, int slope_type, int slope_mag_type) {
   MhdArgs a;
   std::memset(&a, 0, sizeof a);
-  DenseGeom& g = a.g;
-  g.nox = g.noy = g.noz = N / 2; g.ncx = g.ncy = g.ncz = N;
-  g.ox0 = g.oy0 = g.oz0 = 0; g.ox1 = g.oy1 = g.oz1 = N;
-  g.wrapx = g.wrapy = g.wrapz = 1;
-  g.nslot = (long long)(N / 2) * (N / 2) * (N / 2);
+  a.g = box_geom(3, n, shell);
+  const DenseGeom& g = a.g;
   a.uin = uin; a.uout = uout;
   a.P = make_mphys(gamma, smallr, smallc);
   a.P.slope_type = slope_type; a.P.slope_mag_type = slope_mag_type;
-  a.dt_dev = &dt; a.dx = dx; a.nc = (long long)N * N * N;
+  a.dt_dev = &dt; a.dx = dx; a.nc = (long long)g.ncx * g.ncy * g.ncz;
   std::vector<double> W((size_t)MW_NCOMP * a.nc, 0.0), part(5 * 64, 0.0);
   a.W = W.data(); a.part = part.data();
   const long long nb256 = (a.nc + 255) / 256, nb128 = (a.nc + 127) / 128;
@@ -590,20 +609,23 @@ void devnum_mhd_sweep(int N, int r1d, int r2d, int sl, const double* uin, double
   emulate_serial(mhd_update_kernel, a, 8, 256);
 }
 
+void devnum_mhd_sweep(int N, int r1d, int r2d, int sl, const double* uin, double* uout, double dt, double dx, double gamma,
+                      double smallr, double smallc, int slope_type, int slope_mag_type) {
+  const int n[3] = {N, N, N};
+  devnum_mhd_sweep_box(n, k_no_shell, r1d, r2d, sl, uin, uout, dt, dx, gamma, smallr, smallc, slope_type, slope_mag_type);
+}
+
 // the fused dense-box sweep (sweep_dense_kernel: persistent CTAs of 32 x BY threads, cp.async staging, warp shuffles in x, shared
 // memory exchange in y, plane carry in z, fused set_unew / update / set_uold / Courant scan) on a periodic box of N^ndim cells,
 // state in the device layout [nvar][2^ndim][nslot]; nblocks persistent CTAs share the work like on the GPU
-int devnum_sweep_dense(int ndim, int solver, int N, int nblocks, const double* uin, double* uout, double dt, double dx,
-                        int slope_type, double slope_theta, double gamma, double smallr, double smallc, int niter, double* part,
-                        int late) {
+// on a box of n[0] x n[1] x n[2] owned cells (1 beyond ndim), each axis periodic or with a 2-cell ghost shell (box_geom)
+int devnum_sweep_dense_box(int ndim, int solver, const int* n, const int* shell, int nblocks, const double* uin, double* uout,
+                           double dt, double dx, int slope_type, double slope_theta, double gamma, double smallr, double smallc,
+                           int niter, double* part, int late) {
   SweepArgs a;
   std::memset(&a, 0, sizeof a);
-  DenseGeom& g = a.g;
-  g.nox = N / 2; g.noy = ndim > 1 ? N / 2 : 1; g.noz = ndim > 2 ? N / 2 : 1;
-  g.ncx = N; g.ncy = ndim > 1 ? N : 1; g.ncz = ndim > 2 ? N : 1;
-  g.ox0 = g.oy0 = g.oz0 = 0; g.ox1 = N; g.oy1 = ndim > 1 ? N : 1; g.oz1 = ndim > 2 ? N : 1;
-  g.wrapx = 1; g.wrapy = ndim > 1; g.wrapz = ndim > 2;
-  g.nslot = (long long)g.nox * g.noy * g.noz;
+  a.g = box_geom(ndim, n, shell);
+  const DenseGeom& g = a.g;
   a.uin = uin; a.uout = uout;
   a.P = make_phys(gamma, smallr, smallc, slope_theta, 0.8, slope_type, niter);
   a.dt_dev = nullptr; a.dt_val = dt; a.dx = dx; a.inv_dx = 1.0 / dx;
@@ -633,29 +655,41 @@ int devnum_sweep_dense(int ndim, int solver, int N, int nblocks, const double* u
   return nblocks;   // CTAs actually used: part is [4][nblocks]
 }
 
+int devnum_sweep_dense(int ndim, int solver, int N, int nblocks, const double* uin, double* uout, double dt, double dx,
+                        int slope_type, double slope_theta, double gamma, double smallr, double smallc, int niter, double* part,
+                        int late) {
+  const int n[3] = {N, ndim > 1 ? N : 1, ndim > 2 ? N : 1};
+  return devnum_sweep_dense_box(ndim, solver, n, k_no_shell, nblocks, uin, uout, dt, dx, slope_type, slope_theta, gamma, smallr,
+                                smallc, niter, part, late);
+}
+
 // the AMR variant of the dense sweep (AMRV=true: fluxes through faces of refined cells reset to zero, the update ACCUMULATES into
 // uout which already holds unew) on a fully refined periodic level of N^3 cells; refined[8][nslot] = son(cell)>0
-void devnum_sweep_dense_amr(int solver, int N, int nblocks, const double* uin, double* uout, const unsigned char* refined, double dt,
-                            double dx, int slope_type, double gamma, double smallr, double smallc, int niter) {
+void devnum_sweep_dense_amr_box(int solver, const int* n, const int* shell, int nblocks, const double* uin, double* uout,
+                                const unsigned char* refined, double dt, double dx, int slope_type, double gamma, double smallr,
+                                double smallc, int niter) {
   SweepArgs a;
   std::memset(&a, 0, sizeof a);
-  DenseGeom& g = a.g;
-  g.nox = g.noy = g.noz = N / 2; g.ncx = g.ncy = g.ncz = N;
-  g.ox0 = g.oy0 = g.oz0 = 0; g.ox1 = g.oy1 = g.oz1 = N;
-  g.wrapx = g.wrapy = g.wrapz = 1;
-  g.nslot = (long long)(N / 2) * (N / 2) * (N / 2);
+  a.g = box_geom(3, n, shell);
+  const DenseGeom& g = a.g;
   a.uin = uin; a.uout = uout; a.refined = refined;
   a.P = make_phys(gamma, smallr, smallc, 1.5, 0.8, slope_type, niter);
   a.dt_dev = nullptr; a.dt_val = dt; a.dx = dx; a.inv_dx = 1.0 / dx;
   int ex;
   a.dx_pow2 = (std::frexp(dx, &ex) == 0.5) ? 1 : 0;
-  a.ntx = (N + 29) / 30; a.nty = (N + 9) / 10; a.nwork = (long long)a.ntx * a.nty * N;
+  a.ntx = (g.ox1 - g.ox0 + 29) / 30; a.nty = (g.oy1 - g.oy0 + 9) / 10; a.nwork = (long long)a.ntx * a.nty * (g.oz1 - g.oz0);
   if (nblocks > a.nwork) nblocks = (int)a.nwork;
   a.part = nullptr;
 #define SWA(RS) emulate_launch(sweep_dense_kernel<3, RS, -1, 32, 12, true, false>, a, nblocks, 32, 12, SweepSmem<3, 32, 12>::doubles)
   if (solver == RIEMANN_LLF) SWA(RIEMANN_LLF); else if (solver == RIEMANN_EXACT) SWA(RIEMANN_EXACT);
   else if (solver == RIEMANN_ACOUSTIC) SWA(RIEMANN_ACOUSTIC); else if (solver == RIEMANN_HLLC) SWA(RIEMANN_HLLC); else SWA(RIEMANN_HLL);
 #undef SWA
+}
+
+void devnum_sweep_dense_amr(int solver, int N, int nblocks, const double* uin, double* uout, const unsigned char* refined, double dt,
+                            double dx, int slope_type, double gamma, double smallr, double smallc, int niter) {
+  const int n[3] = {N, N, N};
+  devnum_sweep_dense_amr_box(solver, n, k_no_shell, nblocks, uin, uout, refined, dt, dx, slope_type, gamma, smallr, smallc, niter);
 }
 
 
@@ -695,22 +729,21 @@ void devnum_riemann_vec(int solver, int n, const double* ql, const double* qr, d
 }
 
 // sweep3_kernel (sweep_dense3.cuh) on a periodic box of N^3 cells, emulated launch; by in {8, 12, 16}, vec in {0, 1, 2}
-int devnum_sweep3(int solver, int N, int nblocks, const double* uin, double* uout, double dt, double dx, int slope_type,
-                  double slope_theta, double gamma, double smallr, double smallc, int niter, double* part, int by, int vec) {
+// on a box of n[0] x n[1] x n[2] owned cells, each axis periodic or with a 2-cell ghost shell (box_geom)
+int devnum_sweep3_box(int solver, const int* n, const int* shell, int nblocks, const double* uin, double* uout, double dt, double dx,
+                      int slope_type, double slope_theta, double gamma, double smallr, double smallc, int niter, double* part, int by,
+                      int vec) {
   SweepArgs a;
   std::memset(&a, 0, sizeof a);
-  DenseGeom& g = a.g;
-  g.nox = g.noy = g.noz = N / 2; g.ncx = g.ncy = g.ncz = N;
-  g.ox0 = g.oy0 = g.oz0 = 0; g.ox1 = g.oy1 = g.oz1 = N;
-  g.wrapx = g.wrapy = g.wrapz = 1;
-  g.nslot = (long long)g.nox * g.noy * g.noz;
+  a.g = box_geom(3, n, shell);
+  const DenseGeom& g = a.g;
   a.uin = uin; a.uout = uout;
   a.P = make_phys(gamma, smallr, smallc, slope_theta, 0.8, slope_type, niter);
   a.dt_dev = nullptr; a.dt_val = dt; a.dx = dx; a.inv_dx = 1.0 / dx;
   int ex;
   a.dx_pow2 = (std::frexp(dx, &ex) == 0.5) ? 1 : 0;
-  a.ntx = (N + 29) / 30; a.nty = (N + by - 3) / (by - 2);
-  a.nwork = (long long)a.ntx * a.nty * N;
+  a.ntx = (g.ox1 - g.ox0 + 29) / 30; a.nty = (g.oy1 - g.oy0 + by - 3) / (by - 2);   // rgpu_bind_level (rgpu_api.cu)
+  a.nwork = (long long)a.ntx * a.nty * (g.oz1 - g.oz0);
   if (nblocks > a.nwork) nblocks = (int)a.nwork;
   a.part = part; a.refined = nullptr;
 #define S3(RS, BY, VEC) emulate_launch(sweep3_kernel<RS, -1, BY, 1, VEC>, a, nblocks, 32, BY, Sweep3Smem<BY>::doubles)
@@ -725,6 +758,13 @@ int devnum_sweep3(int solver, int N, int nblocks, const double* uin, double* uou
 #undef S3V
 #undef S3
   return nblocks;
+}
+
+int devnum_sweep3(int solver, int N, int nblocks, const double* uin, double* uout, double dt, double dx, int slope_type,
+                  double slope_theta, double gamma, double smallr, double smallc, int niter, double* part, int by, int vec) {
+  const int n[3] = {N, N, N};
+  return devnum_sweep3_box(solver, n, k_no_shell, nblocks, uin, uout, dt, dx, slope_type, slope_theta, gamma, smallr, smallc, niter,
+                           part, by, vec);
 }
 
 void devnum_mhd_cmpdt(int n, const double* u, double dx, double* dt, double gamma, double smallr, double smallc, double cfl) {

@@ -1026,8 +1026,6 @@ def test_sweep3_kernel_emulated_on_the_cpu_equals_oracle(orc, dev, solver, st, N
     dev.devnum_sweep3.argtypes = [C.c_int, C.c_int, C.c_int, dp, dp, C.c_double, C.c_double, C.c_int, C.c_double, C.c_double,
                                   C.c_double, C.c_double, C.c_int, dp, C.c_int, C.c_int]
     from helpers import Case, smooth_state
-    if N & (N - 1):                       # not a power of two: the oracle mesh is a cube of 2^level; use a coarse grid instead
-        pytest.skip("oracle meshes are powers of two")
     level = int(np.log2(N))
     c = Case(3, level, riemann=solver, slope_type=st, slope_theta=1.3)
     d0 = smooth_state(3, N)
@@ -1051,3 +1049,228 @@ def test_sweep3_kernel_emulated_on_the_cpu_equals_oracle(orc, dev, solver, st, N
     assert p4[0].min() * 1.0 == dt_next or min(p4[0].min(), c.p.boxlen / c.p.smallc) == dt_next
     vol = (1.0 / N) ** 3
     assert abs(p4[1].sum() * vol - sums[0]) <= 1e-13 * abs(sums[0]) and abs(p4[2].sum() * vol - sums[1]) <= 1e-13 * abs(sums[1])
+
+
+# ---- non-cubic boxes: per-axis extents, tile counts that do not divide them, thin periodic axes, a ghost shell on one axis ----
+SOLVER_ID = {"llf": 0, "exact": 1, "acoustic": 2, "hllc": 3, "hll": 4}
+IP3 = C.c_int * 3
+
+
+def _box_case(ndim, level, coarse, bound, solver, st, order=1, seed=2):
+    """oracle run set-up on a domain of `coarse` coarse cells (boxlen = coarse[0]: dx = 2^-level) with a box_state that has no
+    symmetry to hide a swapped axis; returns the case, the owned extent in cells, dt and the oracle's new state"""
+    from helpers import Case, box_state
+    c = Case(ndim, level, riemann=solver, slope_type=st, slope_theta=1.3, bound=bound, coarse=coarse, boxlen=float(coarse[0]),
+             order=order, seed=seed)
+    ext = c.mesh.extent(level)
+    c.init_dense(box_state(ndim, ext))
+    dt, _ = c.oracle_courant()
+    unew = c.oracle_godunov(dt, nthreads=1)
+    return c, ext, dt, unew
+
+
+def _check_box_result(c, uout, act, slot, unew, part, nb, ndim):
+    """the owned cells of uout == the oracle's unew, bit for bit; the fused Courant partials give the oracle's next dt"""
+    s = c.mesh.s
+    T = 1 << ndim
+    nv = getattr(c, "nvs", c.nvar)                         # MHD: 11 stored variables
+    U, U0 = unew.reshape(nv, s.ncell), c.u.reshape(nv, s.ncell)
+    moved = 0.0
+    for ind in range(T):
+        cells = s.ncoarse + ind * s.ngridmax + act - 1
+        moved = max(moved, np.abs(U[:, cells] - U0[:, cells]).max())
+        assert np.array_equal(uout[:, ind, slot], U[:, cells]), (ind, float(np.abs(uout[:, ind, slot] - U[:, cells]).max()))
+    assert moved > 1e-4
+    if part is not None:
+        dt_next, sums = c.oracle_courant(unew)
+        p4 = part[:4 * nb].reshape(4, nb)
+        assert min(p4[0].min(), c.p.boxlen / c.p.smallc) == dt_next
+        vol = (2.0 ** -c.level) ** ndim
+        assert abs(p4[1].sum() * vol - sums[0]) <= 1e-13 * abs(sums[0])
+
+
+@pytest.mark.parametrize("coarse,level,bound,solver,st,nblocks,by,vec", [
+    ((3, 2, 1), 4, (0,) * 6, "hllc", 1, 7, 12, 1),              # 48 x 32 x 16
+    ((1, 3, 2), 4, (0,) * 6, "exact", 2, 5, 8, 1),              # 16 x 48 x 32
+    ((2, 1, 3), 4, (0,) * 6, "llf", 8, 5, 16, 1),               # 32 x 16 x 48
+    ((3, 2, 1), 4, (0,) * 6, "hll", 3, 11, 12, 2),
+    ((1, 3, 2), 4, (0,) * 6, "acoustic", 7, 7, 12, 41),         # one-barrier form (sweep_dense4.cuh)
+    ((2, 1, 3), 4, (0,) * 6, "hllc", 2, 7, 12, 12),
+    ((4, 2, 1), 2, (0,) * 6, "hllc", 1, 3, 12, 1),              # 16 x 8 x 4: 4-cell periodic z
+    ((8, 4, 1), 1, (0,) * 6, "llf", 2, 3, 8, 1),                # 16 x 8 x 2: 2-cell periodic z
+    ((1, 4, 8), 1, (0,) * 6, "hllc", 1, 3, 12, 1),              # 2 x 8 x 16: 2-cell periodic x
+    ((3, 2, 1), 3, (1, 1, 0, 0, 0, 0), "hllc", 2, 5, 12, 1),    # 24 x 16 x 8, reflexive x walls: shell on x only
+    ((2, 1, 3), 3, (0, 0, 0, 0, 2, 2), "exact", 1, 5, 8, 1),    # 16 x 8 x 24, outflow z faces: shell on z only
+])
+def test_sweep3_kernel_emulated_on_non_cubic_boxes(orc, dev, coarse, level, bound, solver, st, nblocks, by, vec):
+    """sweep3_kernel / sweep4_kernel on boxes whose three extents differ (each axis the long one once, none a multiple of the
+    30 x (by-2) tile), on thin periodic axes of 2 and 4 cells (the 2-cell halo and the 3-plane z warm-up wrap more than once) and
+    on boxes with a ghost shell on one axis only: the owned cells equal one level step of the oracle bit for bit, and the fused
+    Courant partials give the oracle's next time step.  nblocks never divides the work count."""
+    dev.devnum_sweep3_box.argtypes = [C.c_int, IP3, IP3, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_double,
+                                      C.c_double, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int,
+                                      C.POINTER(C.c_double), C.c_int, C.c_int]
+    from helpers import level_slots
+    c, ext, dt, unew = _box_case(3, level, coarse, bound, solver, st)
+    shell = [int(bound[2 * d] > 0) for d in range(3)]
+    uin, act, slot = level_slots(c.mesh, level, c.u, 5)
+    uout = np.zeros_like(uin)
+    part = np.zeros(4 * 64)
+    nb = dev.devnum_sweep3_box(SOLVER_ID[solver], IP3(*ext), IP3(*shell), nblocks, orc.dptr(uin), orc.dptr(uout), dt,
+                               2.0 ** -level, st, 1.3, 1.4, 1e-10, 1e-10, 10, orc.dptr(part), by, vec)
+    ntx, nty = -(-ext[0] // 30), -(-ext[1] // (by - 2))
+    assert nb == nblocks and (ntx * nty * ext[2]) % nblocks != 0
+    _check_box_result(c, uout, act, slot, unew, part, nb, 3)
+
+
+@pytest.mark.parametrize("ndim,coarse,level,bound,solver,st,nblocks", [
+    (1, (5, 1, 1), 3, (0,) * 6, "hllc", 2, 1),                  # 40 cells
+    (1, (5, 1, 1), 3, (1, 1, 0, 0, 0, 0), "exact", 1, 2),       # 40 cells between walls
+    (2, (3, 2, 1), 4, (0,) * 6, "llf", 8, 5),                   # 48 x 32
+    (2, (3, 2, 1), 4, (0, 0, 1, 1, 0, 0), "hll", 3, 3),         # 48 x 32, walls in y
+    (2, (1, 4, 1), 2, (0,) * 6, "acoustic", 1, 2),              # 4 x 16
+    (3, (3, 2, 1), 3, (0,) * 6, "hllc", 7, 4),                  # 24 x 16 x 8
+    (3, (1, 2, 3), 3, (2, 2, 0, 0, 0, 0), "hllc", 1, 5),        # 8 x 16 x 24, outflow x
+    (3, (8, 4, 1), 1, (0,) * 6, "hllc", 2, 3),                  # 16 x 8 x 2: 2-cell periodic z
+    (3, (1, 4, 2), 2, (0,) * 6, "exact", 1, 2),                 # 4 x 16 x 8: 4-cell periodic x
+])
+def test_dense_sweep_kernel_emulated_on_non_cubic_boxes(orc, dev, ndim, coarse, level, bound, solver, st, nblocks):
+    """sweep_dense_kernel (1-D, 2-D and 3-D forms) on boxes of several coarse cells with different extents per axis, periodic or
+    with a ghost shell on one axis: the owned cells equal one level step of the oracle bit for bit."""
+    dev.devnum_sweep_dense_box.argtypes = [C.c_int, C.c_int, IP3, IP3, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                           C.c_double, C.c_double, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int,
+                                           C.POINTER(C.c_double), C.c_int]
+    from helpers import level_slots
+    c, ext, dt, unew = _box_case(ndim, level, coarse, bound, solver, st)
+    shell = [int(bound[2 * d] > 0) for d in range(3)]
+    uin, act, slot = level_slots(c.mesh, level, c.u, ndim + 2)
+    uout = np.zeros_like(uin)
+    part = np.zeros(4 * 64)
+    nb = dev.devnum_sweep_dense_box(ndim, SOLVER_ID[solver], IP3(*ext), IP3(*shell), nblocks, orc.dptr(uin), orc.dptr(uout), dt,
+                                    2.0 ** -level, st, 1.3, 1.4, 1e-10, 1e-10, 10, orc.dptr(part), 0)
+    _check_box_result(c, uout, act, slot, unew, part, nb, ndim)
+
+
+@pytest.mark.parametrize("coarse,level,bound,r1d,r2d,st", [
+    ((3, 2, 1), 3, (0,) * 6, "roe", "llf", 1),                   # 24 x 16 x 8
+    ((3, 2, 1), 3, (0,) * 6, "hlld", "hlld", 2),
+    ((1, 3, 2), 3, (0,) * 6, "llf", "hll", 1),                   # 8 x 24 x 16
+    ((1, 2, 1), 3, (2, 2, 0, 0, 0, 0), "hlld", "hlld", 1),       # 8 x 16 x 8 between zero-gradient x ends
+    ((8, 4, 1), 1, (0,) * 6, "hlld", "hlld", 2),                 # 16 x 8 x 2: 2-cell periodic z
+    ((1, 4, 2), 2, (0,) * 6, "roe", "llf", 1),                   # 4 x 16 x 8: 4-cell periodic x
+])
+def test_mhd_six_pass_kernels_emulated_on_non_cubic_boxes(orc, dev, coarse, level, bound, r1d, r2d, st):
+    """the six MHD passes of mhd_dense.cuh (cells decoded with ncx / ncy, W indexed [ncz][ncy][ncx]) on boxes of several coarse
+    cells with different extents per axis, periodic or between zero-gradient x ends: the owned cells equal set_unew + godunov_fine
+    of the oracle, bit for bit (both copies of every face field)."""
+    from helpers import MhdCase, level_slots, mhd_box_state
+    dev.devnum_mhd_sweep_box.argtypes = [IP3, IP3, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                         C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int]
+    c = MhdCase(level, riemann=r1d, riemann2d=r2d, slope_type=st, bound=bound, coarse=coarse, boxlen=float(coarse[0]), order=2,
+                seed=3)
+    ext = c.mesh.extent(level)
+    d0 = mhd_box_state(ext)
+    d0[0] *= 1 + 0.2 * (np.random.default_rng(4).standard_normal(d0[0].shape) > 1.3)
+    c.init_dense(d0)
+    dt, _ = c.oracle_courant()
+    dt *= 0.7
+    unew = c.oracle_godunov(dt, nthreads=2)
+    shell = [int(bound[2 * d] > 0) for d in range(3)]
+    uin, act, slot = level_slots(c.mesh, level, c.u, 11)
+    uout = np.zeros_like(uin)
+    dev.devnum_mhd_sweep_box(IP3(*ext), IP3(*shell), orc.MHD_RIEMANN[r1d], orc.MHD_RIEMANN2D[r2d], 0 if st == 0 else 1,
+                             orc.dptr(uin), orc.dptr(uout), dt, 2.0 ** -level, c.p.gamma, c.p.smallr, c.p.smallc, st, st)
+    _check_box_result(c, uout, act, slot, unew, None, 0, 3)
+
+
+@pytest.mark.parametrize("coarse,bound", [((3, 2, 1), (0,) * 6), ((1, 3, 2), (0,) * 6), ((3, 2, 2), (1, 1, 0, 0, 2, 2))])
+def test_amr_tree_walks_across_coarse_cells_equal_oracle(orc, dev, coarse, bound):
+    """amr_get3cubefather / amr_getnborfather of amr_kernels.cuh on a domain of several coarse cells (with and without boundary
+    coarse cells): the level-1 walks decode coarse cells with nx, ny, nz and wrap over the coarse grid; every oct of levels 1-3
+    and every cell of levels 0-2 give the oracle's neighbour cells"""
+    from helpers import Case
+    lev = 3
+    m = Case(3, lev, bound=bound, coarse=coarse, order=2, seed=5).mesh
+    s = m.s
+    assert (s.nx, s.ny, s.nz) == tuple(coarse[d] + (bound[2 * d] > 0) + (bound[2 * d + 1] > 0) for d in range(3))
+    son = np.ascontiguousarray(m.son()[1:], dtype=np.int32)
+    father = np.ascontiguousarray(m.father()[1:], dtype=np.int32)
+    nbor = np.ascontiguousarray(m.nbor()[:, 1:], dtype=np.int32)
+    geo = (3, s.ncoarse, s.ngridmax, s.nx, s.ny, s.nz)
+    L = orc.lib()
+    L.orc_getnborfather.argtypes = [C.POINTER(orc.MeshS), C.c_int, C.c_int, C.POINTER(C.c_int)]
+    buf27, buf7 = (C.c_int * 27)(), (C.c_int * 7)()
+    for l in range(1, lev + 1):
+        act = np.ascontiguousarray(m.active(l), dtype=np.int32)
+        got = np.zeros((len(act), 27), dtype=np.int32)
+        dev.devnum_amr_get3cubefather(*geo, orc.iptr(son), orc.iptr(father), orc.iptr(nbor), len(act), orc.iptr(act), l, orc.iptr(got))
+        ref = np.zeros_like(got)
+        for i, g in enumerate(act):
+            L.orc_get3cubefather(m.ptr, int(father[g - 1]), l, buf27, None)
+            ref[i] = buf27[:27]
+        assert (ref > 0).all() and np.array_equal(got, ref)
+        if l == 1:   # the coarse cells of the domain: the level-1 branch of getnborfather
+            cells = np.arange(1, s.ncoarse + 1, dtype=np.int32)
+        else:
+            prev = m.active(l - 1).astype(np.int64)
+            cells = np.array([s.ncoarse + ind * s.ngridmax + g for g in prev for ind in range(8)], dtype=np.int32)
+        got = np.zeros((len(cells), 7), dtype=np.int32)
+        dev.devnum_amr_getnborfather(*geo, orc.iptr(son), orc.iptr(father), orc.iptr(nbor), len(cells), orc.iptr(cells), l,
+                                     orc.iptr(got))
+        ref = np.zeros_like(got)
+        for i, c in enumerate(cells):
+            L.orc_getnborfather(m.ptr, int(c), l, buf7)
+            ref[i] = buf7[:7]
+        assert np.array_equal(got, ref)
+
+
+@pytest.mark.parametrize("coarse,bound,solver,nblocks", [((3, 2, 1), (0,) * 6, "hllc", 5), ((1, 2, 3), (2, 2, 0, 0, 0, 0), "llf", 7)])
+def test_dense_sweep_amr_variant_emulated_on_non_cubic_boxes(orc, dev, coarse, bound, solver, nblocks):
+    """sweep_dense_kernel<..., AMRV=true> on a 48x32x16 periodic base level and on a 16x32x48 base level between outflow x ends, a
+    scattered tenth of its cells marked refined (son > 0): fluxes through refined faces reset, the update accumulated into a unew
+    that already holds the finer level's refluxes -- equals set_unew + godunov_fine of the oracle on that level, bit for bit"""
+    from helpers import Case, box_state, level_slots
+    dev.devnum_sweep_dense_amr_box.argtypes = [C.c_int, IP3, IP3, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                               C.POINTER(C.c_ubyte), C.c_double, C.c_double, C.c_int, C.c_double, C.c_double,
+                                               C.c_double, C.c_int]
+    lev = 4
+    c = Case(3, lev, riemann=solver, slope_type=1, bound=bound, coarse=coarse, boxlen=float(coarse[0]), order=2, seed=8)
+    ext = c.mesh.extent(lev)
+    c.init_dense(box_state(3, ext))
+    s = c.mesh.s
+    act = c.mesh.active(lev).astype(np.int64)
+    cells = np.concatenate([s.ncoarse + ind * s.ngridmax + act for ind in range(8)])        # 1-based
+    son = c.mesh.son()
+    rng = np.random.default_rng(3)
+    ref_cells = cells[rng.random(len(cells)) < 0.1]
+    son[ref_cells] = 1                                     # marked refined: godfine1 only tests son > 0 on its own level
+    try:
+        dt, _ = c.oracle_courant()
+        L = orc.lib()
+        unew = np.zeros_like(c.u)
+        L.orc_set_unew(C.byref(c.p), c.mesh.ptr, lev, orc.dptr(c.u), orc.dptr(unew))
+        U = unew.reshape(5, s.ncell)
+        U[:, cells - 1] += 1e-3 * rng.standard_normal((5, len(cells))) * (son[cells] == 0)    # refluxes of a finer level
+        start = unew.copy()
+        L.orc_godunov_fine(C.byref(c.p), c.mesh.ptr, lev, dt, orc.dptr(c.u), orc.dptr(unew), 1)
+    finally:
+        son[ref_cells] = 0
+    uin, act_, slot = level_slots(c.mesh, lev, c.u, 5)
+    uout, _, _ = level_slots(c.mesh, lev, start, 5)
+    refined = np.zeros(uin.shape[1:], dtype=np.uint8)
+    for ind in range(8):
+        refined[ind, slot] = np.isin(s.ncoarse + ind * s.ngridmax + act, ref_cells)
+    assert refined.sum() == len(ref_cells) > 0
+    shell = [int(bound[2 * d] > 0) for d in range(3)]
+    unmasked = uout.copy()
+    for mask, out in ((refined, uout), (np.zeros_like(refined), unmasked)):
+        dev.devnum_sweep_dense_amr_box(SOLVER_ID[solver], IP3(*ext), IP3(*shell), nblocks, orc.dptr(uin), orc.dptr(out),
+                                       mask.ctypes.data_as(C.POINTER(C.c_ubyte)), dt, 2.0 ** -lev, 1, 1.4, 1e-10, 1e-10, 10)
+    assert not np.array_equal(unmasked, uout)              # the marks matter
+    Un, Us = unew.reshape(5, s.ncell), start.reshape(5, s.ncell)
+    moved = 0.0
+    for ind in range(8):
+        cc = s.ncoarse + ind * s.ngridmax + act - 1
+        moved = max(moved, np.abs(Un[:, cc] - Us[:, cc]).max())
+        assert np.array_equal(uout[:, ind, slot], Un[:, cc]), (ind, float(np.abs(uout[:, ind, slot] - Un[:, cc]).max()))
+    assert moved > 1e-5
