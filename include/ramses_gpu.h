@@ -72,7 +72,8 @@ typedef struct rgpu_params {
   int poisson;         /* amr_parameters.f90 `poisson`.  1: the acceleration f(1:ncell,1:ndim) of poisson_commons is an INPUT
                         * (rgpu_upload_force; the Poisson solver is out of scope): gravity predictor of ctoprim (umuscl.f90:932-938),
                         * gloc gather of godfine1 (:637-647), add_gravity_source_terms in set_uold (:237-289), gravity term of cmpdt
-                        * (godunov_utils.f90:99-111).  Oct-batch kernel only (rgpu_set_amr), nvar = ndim+2, difmag = 0              */
+                        * (godunov_utils.f90:99-111).  nvar = ndim+2, difmag = 0; oct-batch kernel and the dense sweep (levelmin=
+                        * levelmax levels, AMR base box and patches); with pressure_fix AMR mode only                              */
   double beta_fix;     /* amr_parameters.f90:167 (pressure_fix truncation-error factor)                                          */
 } rgpu_params;
 /* `riemann` / `riemann2d` of the MHD build: iriemann, iriemann2d (hydro/read_hydro_params.f90:190-220) */
@@ -174,8 +175,10 @@ int rgpu_upload_fine(int ilevel);                          /* hydro/interpol_hyd
  * 4-byte flags of the level travel, the state stays on the device for the flag_fine pass.                                  */
 int rgpu_hydro_flag(int ilevel, const double err_grad[3], const double floor[3], int* flag1);
 
-/* Source terms (AMR mode).  rgpu_upload_force: the host array f(1:ncell,1:ndim) of poisson_commons (amr/init_poisson.f90) after
- * force_fine / gravana -- call it whenever the host recomputed the acceleration (rgpu_params.poisson = 1).
+/* Source terms.  rgpu_upload_force: the host array f(1:ncell,1:ndim) of poisson_commons (amr/init_poisson.f90) after
+ * force_fine / gravana -- call it whenever the host recomputed the acceleration (rgpu_params.poisson = 1).  AMR mode: after
+ * rgpu_bind_tree; levelmin=levelmax: after rgpu_bind_level, f is gathered into every bound level, and a sweep or Courant scan of a
+ * level with no upload since its bind fails with RGPU_EINVAL.
  * rgpu_download_pressure_fix: the device-resident divu(1:ncell) / enew(1:ncell) of hydro_commons (hydro/init_hydro.f90:40-42)
  * for diagnostics or a host-side pass that needs them (either pointer may be NULL).                                          */
 /* MHD build in AMR mode: interpol_mag_type of &HYDRO_PARAMS (limiter of the face-field prolongation, interpol_mag

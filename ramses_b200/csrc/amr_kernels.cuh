@@ -701,21 +701,16 @@ __global__ void amr_gravity_src_kernel(const double* __restrict__ uold, double* 
   const int o = i % n, ind = i / n;
   const size_t c = (size_t)ncoarse + (size_t)ind * ngridmax + igrid[o] - 1;
   const double dtl = dt_dev ? *dt_dev : dt;
-  const double d = fmx(unew[c], smallr);
-  double u = 0, v = 0, w = 0;
-  if (ndim > 0) u = unew[(size_t)1 * ncell + c] / d;
-  if (ndim > 1) v = unew[(size_t)2 * ncell + c] / d;
-  if (ndim > 2) w = unew[(size_t)3 * ncell + c] / d;
-  double e_kin = 0.5 * d * (u * u + v * v + w * w);
-  const double e_prim = unew[(size_t)(ndim + 1) * ncell + c] - e_kin;
-  const double d_old = fmx(uold[c], smallr);
-  const double req = 0.0;                               // strict_equilibrium = 0
-  const double fact = (d_old - req) / d * 0.5 * dtl;
-  if (ndim > 0) { u = u + force[c] * fact; unew[(size_t)1 * ncell + c] = d * u; }
-  if (ndim > 1) { v = v + force[(size_t)1 * ncell + c] * fact; unew[(size_t)2 * ncell + c] = d * v; }
-  if (ndim > 2) { w = w + force[(size_t)2 * ncell + c] * fact; unew[(size_t)3 * ncell + c] = d * w; }
-  e_kin = 0.5 * d * (u * u + v * v + w * w);
-  unew[(size_t)(ndim + 1) * ncell + c] = e_prim + e_kin;
+  double mx = 0, my = 0, mz = 0, fx = 0, fy = 0, fz = 0;
+  if (ndim > 0) { mx = unew[(size_t)1 * ncell + c]; fx = force[c]; }
+  if (ndim > 1) { my = unew[(size_t)2 * ncell + c]; fy = force[(size_t)1 * ncell + c]; }
+  if (ndim > 2) { mz = unew[(size_t)3 * ncell + c]; fz = force[(size_t)2 * ncell + c]; }
+  double e = unew[(size_t)(ndim + 1) * ncell + c];
+  gravity_src_cell(unew[c], mx, my, mz, e, fmx(uold[c], smallr), fx, fy, fz, ndim, smallr, dtl);   // strict_equilibrium = 0
+  if (ndim > 0) unew[(size_t)1 * ncell + c] = mx;
+  if (ndim > 1) unew[(size_t)2 * ncell + c] = my;
+  if (ndim > 2) unew[(size_t)3 * ncell + c] = mz;
+  unew[(size_t)(ndim + 1) * ncell + c] = e;
 }
 // add_pdv_source_terms, pressure_fix part (hydro/godunov_fine.f90:294-437): enew -= (gamma-1) e_old div(u) dt, the velocity
 // divergence from the face neighbours in uold (the coarser father cell, 1.5 dx away, where no neighbour oct exists)

@@ -51,6 +51,13 @@ namespace rgpu {
 #define DECL(R) extern template cudaError_t launch_sweep_dense_amr<3, R>(const SweepArgs&, int, cudaStream_t);
 DECL(0) DECL(1) DECL(2) DECL(3) DECL(4)
 #undef DECL
+// poisson: the GRAV instantiations of the dense sweep (sweep_grav_inst_*.cu)
+#define DECL(ND, R, AMRV) extern template cudaError_t launch_sweep_dense_grav<ND, R, AMRV>(const SweepArgs&, int, cudaStream_t);
+DECL(1, 0, false) DECL(1, 1, false) DECL(1, 2, false) DECL(1, 3, false) DECL(1, 4, false)
+DECL(2, 0, false) DECL(2, 1, false) DECL(2, 2, false) DECL(2, 3, false) DECL(2, 4, false)
+DECL(3, 0, false) DECL(3, 1, false) DECL(3, 2, false) DECL(3, 3, false) DECL(3, 4, false)
+DECL(3, 0, true) DECL(3, 1, true) DECL(3, 2, true) DECL(3, 3, true) DECL(3, 4, true)
+#undef DECL
 }  // namespace rgpu
 
 using namespace rgpu;
@@ -133,6 +140,9 @@ struct Level {
   double* d_part = nullptr;          // [5][part_cap]
   double* d_mhdw = nullptr;          // MHD work arrays [MW_NCOMP][ncell_box]
   unsigned char* d_refined = nullptr;  // AMR mode: son(cell)>0 per box cell [2^ndim][nslot]
+  double* d_f = nullptr;             // poisson: the acceleration f [ndim][2^ndim][nslot] (rgpu_upload_force; AMR mode: gathered per call)
+  bool f_valid = false;              // poisson, levelmin=levelmax: f uploaded since the bind
+  double dt_last = 0.0;              // dt of the last godunov_fine (rgpu_set_uold's gravity source term needs it)
   int mhd_nb = 0;                    // CTAs of the MHD update kernel
   int part_cap = 0;
   double* d_dt = nullptr;            // [1] dt used by the next sweep
@@ -336,9 +346,11 @@ __global__ void boundary_kernel(double* __restrict__ u, const BoundArgs b) {
   }
 }
 
-// stand-alone courant_fine scan over the owned cells (hydro/courant_fine.f90:1-159)
-template <int NDIM>
-__global__ void courant_kernel(const double* __restrict__ u, DenseGeom g, Phys P, double dx, double* __restrict__ part) {
+// stand-alone courant_fine scan over the owned cells (hydro/courant_fine.f90:1-159); GRAV (poisson): gg = f, the acceleration in
+// the level-store layout (:75-83)
+template <int NDIM, bool GRAV = false>
+__global__ void courant_kernel(const double* __restrict__ u, DenseGeom g, Phys P, double dx, double* __restrict__ part,
+                               const double* __restrict__ force = nullptr) {
   constexpr int NV = NDIM + 2, T = 1 << NDIM;
   __shared__ double red[4][32];
   const long long nx = g.ox1 - g.ox0, ny = NDIM > 1 ? g.oy1 - g.oy0 : 1, nz = NDIM > 2 ? g.oz1 - g.oz0 : 1;
@@ -351,7 +363,13 @@ __global__ void courant_kernel(const double* __restrict__ u, DenseGeom g, Phys P
 #pragma unroll
     for (int n = 0; n < NV; n++) uu[n] = u[(size_t)n * T * g.nslot + off];
     double ei;
-    const double dtc = cmpdt_cell<NDIM>(uu, dx, P, ei);
+    double gs = -1.0;
+    if (GRAV) {   // the same sum as amr_courant_kernel (amr_kernels.cuh)
+      gs = 0.0;
+#pragma unroll
+      for (int d = 0; d < NDIM; d++) gs = gs + fabs(force[(size_t)d * T * g.nslot + off]);
+    }
+    const double dtc = cmpdt_cell<NDIM>(uu, dx, P, ei, gs);
     my_dt = dtc < my_dt ? dtc : my_dt;
     m0 += uu[0]; m1 += uu[NDIM + 1];
     m2 += ei;
@@ -368,6 +386,42 @@ __global__ void courant_kernel(const double* __restrict__ u, DenseGeom g, Phys P
       const size_t nb = gridDim.x;
       part[0 * nb + blockIdx.x] = v0; part[1 * nb + blockIdx.x] = v1; part[2 * nb + blockIdx.x] = v2; part[3 * nb + blockIdx.x] = v3;
     }
+  }
+}
+
+// set_uold's add_gravity_source_terms (hydro/godunov_fine.f90:159-161,237-289) on the owned cells of a dense level store
+template <int NDIM>
+__global__ void dense_gravity_src_kernel(const double* __restrict__ uold, double* __restrict__ unew, const double* __restrict__ force,
+                                         DenseGeom g, double smallr, double dt) {
+  constexpr int T = 1 << NDIM;
+  const long long nx = g.ox1 - g.ox0, ny = NDIM > 1 ? g.oy1 - g.oy0 : 1, nz = NDIM > 2 ? g.oz1 - g.oz0 : 1;
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i >= nx * ny * nz) return;
+  const int x = g.ox0 + (int)(i % nx), y = NDIM > 1 ? g.oy0 + (int)((i / nx) % ny) : 0, z = NDIM > 2 ? g.oz0 + (int)(i / (nx * ny)) : 0;
+  const long long off = cell_offset<NDIM>(g, x, y, z);
+  const size_t vs = (size_t)T * g.nslot;
+  double un[NDIM + 2], f[NDIM];
+#pragma unroll
+  for (int n = 0; n < NDIM + 2; n++) un[n] = unew[n * vs + off];
+#pragma unroll
+  for (int d = 0; d < NDIM; d++) f[d] = force[d * vs + off];
+  gravity_src_cell(un[0], un[1], un[1 + 1 % NDIM], un[1 + 2 % NDIM], un[NDIM + 1], fmx(uold[off], smallr), f[0], f[1 % NDIM], f[2 % NDIM],
+                   NDIM, smallr, dt);
+#pragma unroll
+  for (int n = 1; n < NDIM + 2; n++) unew[n * vs + off] = un[n];
+}
+
+// AMR patch mode, poisson: the empty shell slots of a refined patch take the f of their father cell (straight injection,
+// hydro/godunov_fine.f90:637-647); force = f[ndim][ncell] of the tree, f = level store [ndim][8][nslot]
+__global__ void amr_fill_shell_force_kernel(const double* __restrict__ force, double* __restrict__ f, const int* __restrict__ shell_father,
+                                            long long nslot, long long ncell, int ndim) {
+  const long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (s >= nslot) return;
+  const int fc = shell_father[s];
+  if (fc <= 0) return;
+  for (int d = 0; d < ndim; d++) {
+    const double v = force[(size_t)d * ncell + fc - 1];
+    for (int is = 0; is < 8; is++) f[((size_t)d * 8 + is) * nslot + s] = v;
   }
 }
 
@@ -510,6 +564,7 @@ void free_level(Level& L) {
   for (auto e : L.ev_c) cudaEventDestroy(e);
   cudaFree(L.d_slot_igrid); cudaFree(L.d_mirror); cudaFree(L.d_u[0]); cudaFree(L.d_u[1]);
   cudaFree(L.d_part); cudaFree(L.d_dt); cudaFree(L.d_out); cudaFree(L.d_hist); cudaFree(L.d_mhdw); cudaFree(L.d_refined);
+  cudaFree(L.d_f);
   for (auto& r : L.regions) cudaFree(r.d_slots);
   for (auto& p : L.peers) { cudaFree(p.d_recv); cudaFree(p.d_emit); cudaFree(p.d_sbuf); cudaFree(p.d_rbuf); }
   L = Level();
@@ -535,10 +590,27 @@ cudaError_t dispatch_sweep_nd(int riemann, const SweepArgs& a, int nb, cudaStrea
     default: return launch_sweep_dense<ND, RIEMANN_HLL>(a, nb, st, by);
   }
 }
+// poisson: the GRAV instantiations (runtime slope switch, default tile height); AMRV: the 3-D AMR variant
+template <int ND, bool AMRV>
+cudaError_t dispatch_sweep_grav(int riemann, const SweepArgs& a, int nb, cudaStream_t st) {
+  switch (riemann) {
+    case RGPU_RIEMANN_LLF: return launch_sweep_dense_grav<ND, RIEMANN_LLF, AMRV>(a, nb, st);
+    case RGPU_RIEMANN_EXACT: return launch_sweep_dense_grav<ND, RIEMANN_EXACT, AMRV>(a, nb, st);
+    case RGPU_RIEMANN_ACOUSTIC: return launch_sweep_dense_grav<ND, RIEMANN_ACOUSTIC, AMRV>(a, nb, st);
+    case RGPU_RIEMANN_HLLC: return launch_sweep_dense_grav<ND, RIEMANN_HLLC, AMRV>(a, nb, st);
+    default: return launch_sweep_dense_grav<ND, RIEMANN_HLL, AMRV>(a, nb, st);
+  }
+}
+inline int need_force(const Level& L) {
+  if (G.p.poisson && !L.f_valid) return fail(RGPU_EINVAL, "poisson: no rgpu_upload_force since the level was bound (the sweep and the Courant "
+                                                         "scan need the acceleration f)");
+  return RGPU_OK;
+}
 
 // zlo/zhi >= 0: sweep only the owned cell planes [zlo, zhi) (Level-0 pipeline; no Courant partials then)
 // part: 0 whole level, 1 interior, 2 frame (Level::wk_int / wk_frame; Courant partials of 1 and 2 share one array)
-int launch_sweep(Level& L, int zlo = -1, int zhi = -1, int part = 0) {
+// gsrc (poisson): set_uold's gravity source term and the gravity term of the Courant scan are fused into the sweep
+int launch_sweep(Level& L, int zlo = -1, int zhi = -1, int part = 0, bool gsrc = false) {
   if (G.p.mhd) {
     MhdArgs m{};
     m.uin = L.d_u[L.cur]; m.uout = L.d_u[1 - L.cur]; m.g = L.g; m.P = G.mphys; m.dt_dev = L.d_dt; m.dx = L.dx;
@@ -557,11 +629,13 @@ int launch_sweep(Level& L, int zlo = -1, int zhi = -1, int part = 0) {
     L.launches += 6;
     return RGPU_OK;
   }
+  { const int rc = need_force(L); if (rc) return rc; }
   SweepArgs a{};
   a.uin = L.d_u[L.cur];
   a.uout = L.d_u[1 - L.cur];
   a.g = L.g;
   a.P = G.phys;
+  if (G.p.poisson) { a.force = L.d_f; a.gsrc = gsrc ? 1 : 0; }
   a.dt_dev = L.d_dt;
   if (L.dt_by_value > 0.0) { a.dt_dev = nullptr; a.dt_val = L.dt_by_value; }
   a.dx = L.dx;
@@ -589,7 +663,12 @@ int launch_sweep(Level& L, int zlo = -1, int zhi = -1, int part = 0) {
   }
   if (G.timing) cudaEventRecord(G.ev0, G.stream);
   cudaError_t e;
-  if (G.p.ndim == 1) e = dispatch_sweep_nd<1>(G.p.riemann, a, nblocks, G.stream, L.by);
+  if (G.p.poisson) {   // round-1 kernel with gravity (3-D: variant 0, FAST ignored; rgpu_bind_level)
+    if (G.p.ndim == 1) e = dispatch_sweep_grav<1, false>(G.p.riemann, a, nblocks, G.stream);
+    else if (G.p.ndim == 2) e = dispatch_sweep_grav<2, false>(G.p.riemann, a, nblocks, G.stream);
+    else e = dispatch_sweep_grav<3, false>(G.p.riemann, a, nblocks, G.stream);
+  }
+  else if (G.p.ndim == 1) e = dispatch_sweep_nd<1>(G.p.riemann, a, nblocks, G.stream, L.by);
   else if (G.p.ndim == 2) e = dispatch_sweep_nd<2>(G.p.riemann, a, nblocks, G.stream, L.by);
   else if (L.variant && G.p.fast) {
     switch (G.p.riemann) {
@@ -649,7 +728,13 @@ int launch_courant(Level& L, double dt_cap, double* hist_slot) {
     L.launches++;
     return launch_reduce(L, nb, dt_cap, hist_slot);
   }
-  if (G.p.ndim == 1) courant_kernel<1><<<nb, 256, 0, G.stream>>>(L.d_u[L.cur], L.g, G.phys, L.dx, L.d_part);
+  if (G.p.poisson) {   // gg = f (courant_fine.f90:75-83)
+    const int rc = need_force(L); if (rc) return rc;
+    if (G.p.ndim == 1) courant_kernel<1, true><<<nb, 256, 0, G.stream>>>(L.d_u[L.cur], L.g, G.phys, L.dx, L.d_part, L.d_f);
+    else if (G.p.ndim == 2) courant_kernel<2, true><<<nb, 256, 0, G.stream>>>(L.d_u[L.cur], L.g, G.phys, L.dx, L.d_part, L.d_f);
+    else courant_kernel<3, true><<<nb, 256, 0, G.stream>>>(L.d_u[L.cur], L.g, G.phys, L.dx, L.d_part, L.d_f);
+  }
+  else if (G.p.ndim == 1) courant_kernel<1><<<nb, 256, 0, G.stream>>>(L.d_u[L.cur], L.g, G.phys, L.dx, L.d_part);
   else if (G.p.ndim == 2) courant_kernel<2><<<nb, 256, 0, G.stream>>>(L.d_u[L.cur], L.g, G.phys, L.dx, L.d_part);
   else courant_kernel<3><<<nb, 256, 0, G.stream>>>(L.d_u[L.cur], L.g, G.phys, L.dx, L.d_part);
   CUDA_OK(cudaGetLastError());
@@ -828,6 +913,17 @@ int amr_godunov_dense(AmrLevel& A, int ilevel, double dt, const double* dt_dev) 
   amr_gather_slots_kernel<<<nb, nthr, 0, G.stream>>>(G.d_uold, L.d_u[0], L.d_slot_igrid, L.nslot, G.ncoarse, G.ngridmax, G.ncell, G.p.nvar, T_());
   amr_gather_slots_kernel<<<nb, nthr, 0, G.stream>>>(G.d_unew, L.d_u[1], L.d_slot_igrid, L.nslot, G.ncoarse, G.ngridmax, G.ncell, G.p.nvar, T_());
   CUDA_OK(cudaGetLastError());
+  if (G.p.poisson) {   // f of every oct of the box (the host may upload a new f every step); a patch's empty shell slots take the
+                       // f of their father cell (gloc gather, godunov_fine.f90:637-647)
+    amr_gather_slots_kernel<<<nb, nthr, 0, G.stream>>>(G.d_force, L.d_f, L.d_slot_igrid, L.nslot, G.ncoarse, G.ngridmax, G.ncell, G.p.ndim, T_());
+    CUDA_OK(cudaGetLastError());
+    A.launches++;
+    if (A.patch) {
+      amr_fill_shell_force_kernel<<<nb, nthr, 0, G.stream>>>(G.d_force, L.d_f, A.d_shell_father, L.nslot, G.ncell, G.p.ndim);
+      CUDA_OK(cudaGetLastError());
+      A.launches++;
+    }
+  }
   if (A.patch) {   // ghost shell: prolongation from level l-1 (what godfine1 does for every missing neighbour oct, :583-593)
     const long long n = L.nslot * G.p.nvar;
     if (G.interpol_var != 0 || G.interpol_type == 4)
@@ -845,6 +941,10 @@ int amr_godunov_dense(AmrLevel& A, int ilevel, double dt, const double* dt_dev) 
   a.dx_pow2 = (std::frexp(L.dx, &ex) == 0.5) ? 1 : 0;
   a.ntx = L.ntx; a.nty = L.nty; a.nwork = L.nwork; a.part = nullptr; a.refined = L.d_refined;
   cudaError_t e;
+  if (G.p.poisson) {   // predictor only: set_uold and courant_fine apply the gravity terms through their list kernels
+    a.force = L.d_f; a.gsrc = 0;
+    e = dispatch_sweep_grav<3, true>(G.p.riemann, a, L.nblocks, G.stream);
+  } else
   switch (G.p.riemann) {
     case RGPU_RIEMANN_LLF: e = launch_sweep_dense_amr<3, RIEMANN_LLF>(a, L.nblocks, G.stream); break;
     case RGPU_RIEMANN_EXACT: e = launch_sweep_dense_amr<3, RIEMANN_EXACT>(a, L.nblocks, G.stream); break;
@@ -864,6 +964,7 @@ int amr_godunov_dense(AmrLevel& A, int ilevel, double dt, const double* dt_dev) 
     s.P = G.phys; s.dt = dt; s.dt_dev = dt_dev; s.dx = A.dx; s.inv_dx = 1.0 / A.dx; s.dx_pow2 = a.dx_pow2;
     s.interpol_type = G.interpol_type; s.interpol_var = G.interpol_var; s.difmag = 0.0; s.nps = 0;
     s.flux_only = 1; s.rflux_index = A.d_surf_io;
+    s.force = G.p.poisson ? G.d_force : nullptr; s.pfix = 0; s.nvr = G.nvn;   // the refluxed faces carry the gravity predictor
     e = dispatch_amr_nd<3>(G.p.riemann, s, G.stream);
     if (e != cudaSuccess) return fail(RGPU_ECUDA, "patch surface flux launch: %s", cudaGetErrorString(e));
     A.launches++;
@@ -1530,6 +1631,11 @@ static int alloc_dense_store(Level& L, int ncpu, int nboundary, const int* bound
   CUDA_OK(cudaMalloc(&L.d_u[1], sizeof(double) * np * nslot));
   CUDA_OK(cudaMemset(L.d_u[0], 0, sizeof(double) * np * nslot));
   CUDA_OK(cudaMemset(L.d_u[1], 0, sizeof(double) * np * nslot));
+  L.f_valid = false;
+  if (G.p.poisson) {
+    CUDA_OK(cudaMalloc(&L.d_f, sizeof(double) * nd * T_() * nslot));
+    CUDA_OK(cudaMemset(L.d_f, 0, sizeof(double) * nd * T_() * nslot));
+  }
   L.regions.resize(nboundary);
   for (int b = 0; b < nboundary; b++) {
     L.regions[b].type = boundary_type[b];
@@ -1590,10 +1696,11 @@ static int alloc_dense_store(Level& L, int ncpu, int nboundary, const int* bound
   // ---- tile decomposition of the owned range ----------------------------------------------------
   const int bx = 32;
   int by = tile_by_default(nd, G.p.riemann);
-  if (nd == 3) { const char* e = getenv("RGPU_BY3"); if (e) { const int v = atoi(e); if (v == 8 || v == 12 || v == 16) by = v; } }
+  // poisson: the GRAV instantiations exist for the default tile height of the round-1 kernel only (variant 0, FAST ignored)
+  if (nd == 3 && !G.p.poisson) { const char* e = getenv("RGPU_BY3"); if (e) { const int v = atoi(e); if (v == 8 || v == 12 || v == 16) by = v; } }
   int minb = 1;
   L.variant = 0;
-  if (nd == 3 && !G.p.mhd && !G.amr) {   // plain dense 3-D sweep: round-2 kernel; RGPU_SWEEP=old|<variant> for tuning runs
+  if (nd == 3 && !G.p.mhd && !G.amr && !G.p.poisson) {   // plain dense 3-D sweep: round-2 kernel; RGPU_SWEEP=old|<variant> for tuning runs
     // the two-barrier loop (sweep3_kernel, three scalar branch-free solves); profiles/tune_sweep.py times the variants
     L.variant = SWEEP3_DEFAULT_VARIANT;
     const char* e = getenv("RGPU_SWEEP");
@@ -1676,7 +1783,7 @@ int rgpu_bind_level(int ilevel, int ngrid_active, const int* igrid_active, int n
     const char* env = getenv("RGPU_AMR_DENSE");
     const char* envp = getenv("RGPU_AMR_PATCH");
     const bool eligible = !(env && atoi(env) == 0) && G.p.ndim == 3 && !G.p.mhd && !(G.p.difmag > 0.0) && G.p.nvar == G.p.ndim + 2 &&
-                          ngrid_active > 0 && !src_terms();   // gravity / pressure_fix: oct-batch kernel only
+                          ngrid_active > 0 && !G.p.pressure_fix;   // pressure_fix: oct-batch kernel only (poisson: GRAV variant)
     const bool base = eligible && A.nent == 0 && ncpu == 1;   // multi-rank AMR keeps the oct-batch kernel (tested path)
     // a refined level whose octs form a Cartesian box (nested / zoom refinement): dense kernel on the box + a prolongated
     // ghost shell; the octs at its surface go through the oct-batch kernel once more for the refluxed faces only
@@ -1722,9 +1829,11 @@ int rgpu_bind_level(int ilevel, int ngrid_active, const int* igrid_active, int n
   }
   if (G.p.mhd && G.p.ndim != 3)
     return fail(RGPU_EUNSUPPORTED, "MHD build, NDIM=%d: built in AMR mode only -- call rgpu_set_amr(1, interpol_type, 0) after rgpu_init", G.p.ndim);
-  if (G.p.difmag > 0.0 || (!G.p.mhd && G.p.nvar != G.p.ndim + 2) || src_terms())
-    return fail(RGPU_EUNSUPPORTED, "difmag>0 (cmpdivu/consup), passive scalars (nvar>ndim+2), poisson and pressure_fix are built in the oct-batch "
-                                   "kernel only: call rgpu_set_amr(1, interpol_type, 0) after rgpu_init (works for levelmin=levelmax runs too)");
+  // poisson runs through the dense sweep's GRAV instantiation (rgpu_init admits it for nvar = ndim+2, difmag = 0 only)
+  if (G.p.difmag > 0.0 || (!G.p.mhd && G.p.nvar != G.p.ndim + 2) || G.p.pressure_fix)
+    return fail(RGPU_EUNSUPPORTED, "difmag>0 (cmpdivu/consup), passive scalars (nvar>ndim+2) and pressure_fix (also with poisson) are built in "
+                                   "the oct-batch kernel only: call rgpu_set_amr(1, interpol_type, 0) after rgpu_init (works for levelmin=levelmax "
+                                   "runs too)");
   Level& L = G.lev[ilevel];
   if (L.bound) free_level(L);
   {
@@ -1779,17 +1888,19 @@ int rgpu_host_unregister(void* ptr) {
   return RGPU_OK;
 }
 
-static int upload_into(Level& L, const double* host, double* dst) {
+// host array [nv][ncell] (nv < 0: the G.nvs state variables) -> level store
+static int upload_into(Level& L, const double* host, double* dst, int nv = -1) {
   const int T = T_();
   const long long gspan = (long long)L.gmax - L.gmin + 1;
   const size_t ncell = (size_t)G.ncoarse + (size_t)T * G.ngridmax;
-  for (int iv = 0; iv < G.nvs; iv++)
+  if (nv < 0) nv = G.nvs;
+  for (int iv = 0; iv < nv; iv++)
     for (int ind = 0; ind < T; ind++) {
       const double* src = host + (size_t)iv * ncell + G.ncoarse + (size_t)ind * G.ngridmax + (L.gmin - 1);
       CUDA_OK(cudaMemcpyAsync(L.d_mirror + ((size_t)iv * T + ind) * gspan, src, sizeof(double) * gspan, cudaMemcpyHostToDevice, G.stream));
     }
   const int nthr = 256;
-  gather_slots_kernel<<<(unsigned)((L.nslot + nthr - 1) / nthr), nthr, 0, G.stream>>>(L.d_mirror, dst, L.d_slot_igrid, L.nslot, L.gmin, gspan, (int)nplanes_());
+  gather_slots_kernel<<<(unsigned)((L.nslot + nthr - 1) / nthr), nthr, 0, G.stream>>>(L.d_mirror, dst, L.d_slot_igrid, L.nslot, L.gmin, gspan, nv * T);
   CUDA_OK(cudaGetLastError());
   L.launches++;
   return RGPU_OK;
@@ -1971,6 +2082,7 @@ int rgpu_godunov_fine_dev(int ilevel, double dt) {
   L->dt_by_value = 0.0;
   if (rc) return rc;
   L->unew_valid = true;
+  L->dt_last = dt;
   return RGPU_OK;
 }
 
@@ -1981,6 +2093,21 @@ int rgpu_set_uold(int ilevel) {
   }
   Level* L; int rc = check_level(ilevel, &L); if (rc) return rc;
   if (!L->unew_valid) return fail(RGPU_EINVAL, "set_uold before set_unew/godunov_fine");
+  if (G.p.poisson) {   // add_gravity_source_terms on the owned cells of unew (godunov_fine.f90:159-161)
+    if (!(L->dt_last > 0)) return fail(RGPU_EINVAL, "set_uold with poisson before godunov_fine (dtnew(ilevel) unknown)");
+    rc = need_force(*L); if (rc) return rc;
+    long long n = L->g.ox1 - L->g.ox0;
+    if (G.p.ndim > 1) n *= L->g.oy1 - L->g.oy0;
+    if (G.p.ndim > 2) n *= L->g.oz1 - L->g.oz0;
+    const unsigned nb = (unsigned)((n + 127) / 128);
+    const double* uo = L->d_u[L->cur];
+    double* un = L->d_u[1 - L->cur];
+    if (G.p.ndim == 1) dense_gravity_src_kernel<1><<<nb, 128, 0, G.stream>>>(uo, un, L->d_f, L->g, G.p.smallr, L->dt_last);
+    else if (G.p.ndim == 2) dense_gravity_src_kernel<2><<<nb, 128, 0, G.stream>>>(uo, un, L->d_f, L->g, G.p.smallr, L->dt_last);
+    else dense_gravity_src_kernel<3><<<nb, 128, 0, G.stream>>>(uo, un, L->d_f, L->g, G.p.smallr, L->dt_last);
+    CUDA_OK(cudaGetLastError());
+    L->launches++;
+  }
   // uold <- unew on the active cells (godunov_fine.f90:193-197); shells keep their uold values
   rc = carry_shells(*L, L->d_u[L->cur], L->d_u[1 - L->cur]); if (rc) return rc;
   L->cur = 1 - L->cur;
@@ -2063,7 +2190,9 @@ int rgpu_godunov_fine(int ilevel, double dt, const double* uold, double* unew) {
   Level* L; int rc = check_level(ilevel, &L); if (rc) return rc;
   if (!uold || !unew) return fail(RGPU_EINVAL, "null state array");
   if (!(dt > 0)) return fail(RGPU_EINVAL, "dt=%g", dt);
+  rc = need_force(*L); if (rc) return rc;
   CUDA_OK(cudaMemcpyAsync(L->d_dt, &dt, sizeof(double), cudaMemcpyHostToDevice, G.stream));
+  L->dt_last = dt;   // poisson: unew = uold + dF with the gravity predictor; the host's set_uold adds the source term
   if (!L->slabs.empty() && G.pipeline && !G.timing) return godunov_fine_pipelined(*L, uold, unew);
   rc = upload_into(*L, uold, L->d_u[L->cur]); if (rc) return rc;
   rc = launch_sweep(*L); if (rc) return rc;
@@ -2104,9 +2233,9 @@ int rgpu_level_steps(int ilevel, int nstep, double* dt_hist, double sums_last[3]
     if (ovl) {
       // interior tiles read owned cells only: they run while the exchange of the previous step (stream s_x) fills the ghost
       // shells; the frame (outer tile ring + plane caps) waits for it.  Same kernel, same arithmetic, two launches.
-      rc = launch_sweep(*L, -1, -1, 1); if (rc) return rc;
+      rc = launch_sweep(*L, -1, -1, 1, true); if (rc) return rc;
       CUDA_OK(cudaStreamWaitEvent(G.stream, L->ev_x, 0));
-      rc = launch_sweep(*L, -1, -1, 2); if (rc) return rc;
+      rc = launch_sweep(*L, -1, -1, 2, true); if (rc) return rc;
       rc = launch_reduce(*L, 2 * L->nblocks, dt_cap, L->d_hist + s + 1); if (rc) return rc;
       rc = carry_shells(*L, L->d_u[L->cur], L->d_u[1 - L->cur], false); if (rc) return rc;
       L->cur = 1 - L->cur;
@@ -2122,7 +2251,7 @@ int rgpu_level_steps(int ilevel, int nstep, double* dt_hist, double sums_last[3]
       CUDA_OK(cudaEventRecord(L->ev_x, G.s_x));
       continue;
     }
-    rc = launch_sweep(*L); if (rc) return rc;                                        // set_unew + godunov_fine + set_uold  :333,:388,:423
+    rc = launch_sweep(*L, -1, -1, 0, true); if (rc) return rc;                       // set_unew + godunov_fine + set_uold  :333,:388,:423
     rc = launch_reduce(*L, L->nblocks, dt_cap, L->d_hist + s + 1); if (rc) return rc;  // courant_fine of the next step
     rc = carry_shells(*L, L->d_u[L->cur], L->d_u[1 - L->cur], !fused); if (rc) return rc;
     L->cur = 1 - L->cur;
@@ -2320,9 +2449,23 @@ int rgpu_set_boundary_var(int ibound, const double* var) {
   return RGPU_OK;
 }
 int rgpu_upload_force(const double* f) {
-  if (!G.init || !G.amr) return fail(RGPU_EINVAL, "rgpu_upload_force needs AMR mode (rgpu_set_amr)");
+  if (!G.init) return fail(RGPU_EINVAL, "rgpu_init has not been called");
   if (!G.p.poisson) return fail(RGPU_EINVAL, "rgpu_upload_force: rgpu_params.poisson is 0");
-  if (!G.d_force || !f) return fail(RGPU_EINVAL, "bind the tree first / null f");
+  if (!f) return fail(RGPU_EINVAL, "null f");
+  if (!G.amr) {   // levelmin=levelmax: gather f(1:ncell,1:ndim) into the f store of every bound dense level (no full-size mirror)
+    int n = 0;
+    for (int l = 1; l <= MAXLEVEL; l++) {
+      Level& L = G.lev[l];
+      if (!L.bound || !L.dense || !L.d_f) continue;
+      const int rc = upload_into(L, f, L.d_f, G.p.ndim); if (rc) return rc;
+      L.f_valid = true;
+      n++;
+    }
+    if (n == 0) return fail(RGPU_EINVAL, "rgpu_upload_force: bind a level first");
+    CUDA_OK(cudaStreamSynchronize(G.stream));
+    return RGPU_OK;
+  }
+  if (!G.d_force) return fail(RGPU_EINVAL, "bind the tree first");
   CUDA_OK(cudaMemcpyAsync(G.d_force, f, sizeof(double) * G.p.ndim * G.ncell, cudaMemcpyHostToDevice, G.stream));
   CUDA_OK(cudaStreamSynchronize(G.stream));
   return RGPU_OK;

@@ -70,6 +70,11 @@ struct SweepArgs {
   const unsigned char* refined;  // [2^ndim][nslot] son(cell)>0: fluxes through faces of refined cells are reset to zero
                                  // and the update ACCUMULATES into uout (= unew, which already holds the refluxes of the
                                  // finer level) instead of starting from uin
+  // poisson (GRAV instantiation): the acceleration f of poisson_commons in the level-store layout [ndim][2^ndim][nslot]
+  // (addressed like uin); every converted cell gets the gravity predictor (hydro/umuscl.f90:932-938)
+  const double* force;
+  int gsrc;                   // 1: set_uold's add_gravity_source_terms is fused into the update and the Courant scan of the
+                              // new state uses sum|f| (rgpu_level_steps: f stays fixed over the steps of the call)
 };
 
 __device__ __forceinline__ int wrap_or_clamp(int c, int n, int wrap) {
@@ -172,7 +177,7 @@ __device__ __forceinline__ void cp_async8(double* smem_dst, const double* gsrc) 
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
 #endif
 
-template <int NDIM, int BX, int BY>
+template <int NDIM, int BX, int BY, bool GRAV = false>
 struct SweepSmem {
   static constexpr int NV = NDIM + 2;
   static constexpr int HY = (NDIM > 1) ? 1 : 0;
@@ -183,19 +188,23 @@ struct SweepSmem {
   static constexpr int NT = BX * BY;
   static constexpr size_t ring = (size_t)NRING * NQ * QY * QX;
   static constexpr size_t stage = HZ ? (size_t)NV * QY * QX : 0;
+  static constexpr size_t fstage = (HZ && GRAV) ? (size_t)NDIM * QY * QX : 0;   // f of the staged plane
   static constexpr size_t exq = HY ? (size_t)NV * NT : 0;  // qm_y
   static constexpr size_t exf = HY ? (size_t)NV * NT : 0;  // Fy
   static constexpr size_t carry = HZ ? (size_t)3 * NV * NT : 0;
-  static constexpr size_t doubles = ring + stage + exq + exf + carry;
+  static constexpr size_t doubles = ring + stage + fstage + exq + exf + carry;
 };
 
 // LATE (experimental, not dispatched by the product yet; exercised by tests/host_numerics): the x/y part of the update of plane k
 // is finished after the FIRST barrier of plane k+1 instead of after a third barrier of its own -- the y fluxes of the row above
 // are complete by then -- so the plane loop has two CTA barriers instead of three.  Same arithmetic in the same order.
-template <int NDIM, int RIEMANN, int SLOPE, int BX, int BY, bool AMRV = false, bool LATE = false>
+// GRAV (poisson): the gravity predictor with f = a.force in ctoprim of every converted cell and, when a.gsrc is set, set_uold's
+// add_gravity_source_terms in the update plus the gravity term of the fused Courant scan.
+template <int NDIM, int RIEMANN, int SLOPE, int BX, int BY, bool AMRV = false, bool LATE = false, bool GRAV = false>
 __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs a) {
   static_assert(!(LATE && AMRV), "the late-update variant exists for the plain dense sweep only");
-  using S = SweepSmem<NDIM, BX, BY>;
+  static_assert(!(LATE && GRAV), "the late-update variant exists for the plain dense sweep only");
+  using S = SweepSmem<NDIM, BX, BY, GRAV>;
   constexpr int NV = S::NV, HY = S::HY, HZ = S::HZ, QX = S::QX, QY = S::QY, NQ = S::NQ, NT = S::NT;
   constexpr int TXO = BX - 2;                 // owned cells per tile in x
   constexpr int TYO = HY ? BY - 2 : 1;
@@ -209,7 +218,8 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
 #endif
   double* qring = smem;                        // [NRING][NQ][QY][QX]
   double* stage = qring + S::ring;             // [NV][QY][QX] raw conserved state of the next plane
-  double* exq = stage + S::stage;              // [NV][NT] qm_y
+  double* fstg = stage + S::stage;             // GRAV: [NDIM][QY][QX] f of the next plane
+  double* exq = fstg + S::fstage;              // [NV][NT] qm_y
   double* exf = exq + S::exq;                  // [NV][NT] Fy
   double* carry = exf + S::exf;                // [3][NV][NT]: qm_z, Fz, partial update of the previous plane
   __shared__ double red[4][NT / 32];
@@ -264,8 +274,8 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
       const int zc = wrap_or_clamp(z, g.ncz, g.wrapz);
       return (long long)((zc & 1) << 2) * g.nslot + (long long)g.nox * g.noy * (zc >> 1);
     };
-    // ctoprim (hydro/umuscl.f90:861) of one cell into ring slot `slot`
-    auto to_ring = [&](const double* u, int slot, int i) {
+    // ctoprim (hydro/umuscl.f90:861) of one cell into ring slot `slot`; fg: GRAV: the cell's f
+    auto to_ring = [&](const double* u, const double* fg, int slot, int i) {
       double q[NV];
       const double r = fmx(u[0], P.smallr);
       const double oneoverrho = rcp_rn(r);
@@ -277,9 +287,16 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
       if (NDIM > 2) { q[3] = u[3] * oneoverrho; eken = eken + 0.5 * q[3] * q[3]; }
       const double eint = fmx(u[NDIM + 1] * oneoverrho - eken - 0.0, P.smalle);
       q[NDIM + 1] = (P.gamma - 1.0) * r * eint;
-      q[1] = q[1] + 0.0;                       // gravity predictor with gloc = 0 (:932-938): -0 -> +0
-      if (NDIM > 1) q[2] = q[2] + 0.0;
-      if (NDIM > 2) q[3] = q[3] + 0.0;
+      if (GRAV) {                              // gravity predictor (:932-938)
+        const double dtxhalf = dt * 0.5;
+        q[1] = q[1] + fg[0] * dtxhalf;
+        if (NDIM > 1) q[2] = q[2] + fg[1 % NDIM] * dtxhalf;
+        if (NDIM > 2) q[3] = q[3] + fg[2 % NDIM] * dtxhalf;
+      } else {
+        q[1] = q[1] + 0.0;                     // gravity predictor with gloc = 0 (:932-938): -0 -> +0
+        if (NDIM > 1) q[2] = q[2] + 0.0;
+        if (NDIM > 2) q[3] = q[3] + 0.0;
+      }
       double* qs = qring + (size_t)slot * NQ * PL + i;
 #pragma unroll
       for (int n = 0; n < NV; n++) qs[n * PL] = q[n];
@@ -292,13 +309,17 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
         const int i = tid + j * NT;
         if (i >= PL) break;
         const long long off = offxy[j] + zo;
-        double u[NV];
+        double u[NV], fg[NDIM];
 #pragma unroll
         for (int n = 0; n < NV; n++) u[n] = __ldg(a.uin + n * vstride + off);
-        to_ring(u, slot, i);
+        if (GRAV) {
+#pragma unroll
+          for (int d = 0; d < NDIM; d++) fg[d] = __ldg(a.force + d * vstride + off);
+        }
+        to_ring(u, fg, slot, i);
       }
     };
-    auto stage_plane_async = [&](int z) {     // raw u of plane z -> staging buffer (cp.async, no registers)
+    auto stage_plane_async = [&](int z) {     // raw u (and f) of plane z -> staging buffer (cp.async, no registers)
       const long long zo = zoff(z);
 #pragma unroll
       for (int j = 0; j < NOWN; j++) {
@@ -307,15 +328,23 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
         const long long off = offxy[j] + zo;
 #pragma unroll
         for (int n = 0; n < NV; n++) cp_async8(stage + n * PL + i, a.uin + n * vstride + off);
+        if (GRAV) {
+#pragma unroll
+          for (int d = 0; d < NDIM; d++) cp_async8(fstg + d * PL + i, a.force + d * vstride + off);
+        }
       }
     };
     auto stage_to_ring = [&](int slot) {       // each thread converts the cells it staged itself
       cp_async_wait_all();
       for (int i = tid; i < PL; i += NT) {
-        double u[NV];
+        double u[NV], fg[NDIM];
 #pragma unroll
         for (int n = 0; n < NV; n++) u[n] = stage[n * PL + i];
-        to_ring(u, slot, i);
+        if (GRAV) {
+#pragma unroll
+          for (int d = 0; d < NDIM; d++) fg[d] = fstg[d * PL + i];
+        }
+        to_ring(u, fg, slot, i);
       }
     };
 
@@ -602,11 +631,24 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
         }
         if (have) {
           const long long off = cell_offset<NDIM>(g, cx, cy, HZ ? k - 1 : 0);
+          double gsum = -1.0;                  // no gravity term in the Courant scan
+          if (GRAV && a.gsrc) {                // set_uold: add_gravity_source_terms (godunov_fine.f90:159-161); courant gg = f
+            // d_old = MAX(uold(rho), smallr): the q[0] that ctoprim put into the ring for this cell, re-read from uold
+            double fc[NDIM];
+#pragma unroll
+            for (int d = 0; d < NDIM; d++) fc[d] = __ldg(a.force + d * vstride + off);
+            const double d_old = fmx(__ldg(a.uin + off), P.smallr);
+            gravity_src_cell(unew_[0], unew_[1], unew_[1 + 1 % NDIM], unew_[1 + 2 % NDIM], unew_[NDIM + 1], d_old, fc[0],
+                             fc[1 % NDIM], fc[2 % NDIM], NDIM, P.smallr, dt);
+            gsum = 0.0;
+#pragma unroll
+            for (int d = 0; d < NDIM; d++) gsum = gsum + fabs(fc[d]);
+          }
 #pragma unroll
           for (int n = 0; n < NV; n++) a.uout[n * vstride + off] = unew_[n];   // set_uold: uold = unew
           // fused courant_fine of the new state (hydro/courant_fine.f90:96-123)
           double ei;
-          const double dtc = cmpdt_cell<NDIM>(unew_, a.dx, P, ei);
+          const double dtc = cmpdt_cell<NDIM>(unew_, a.dx, P, ei, gsum);
           my_dt = dtc < my_dt ? dtc : my_dt;
           my_mass += unew_[0];
           my_etot += unew_[NDIM + 1];
@@ -707,6 +749,23 @@ cudaError_t launch_sweep_dense(const SweepArgs& a, int nblocks, cudaStream_t st,
   if (a.P.slope_type == 1) return launch_sweep_dense_s<NDIM, RIEMANN, 1>(a, nblocks, st, by);
   if (a.P.slope_type == 2) return launch_sweep_dense_s<NDIM, RIEMANN, 2>(a, nblocks, st, by);
   return launch_sweep_dense_s<NDIM, RIEMANN, -1>(a, nblocks, st, by);
+}
+// poisson (GRAV): one instantiation per dimension and solver with the runtime slope switch and the default tile height, plus
+// the 3-D AMR variant (sweep_grav_inst_*.cu)
+template <int NDIM, int RIEMANN, bool AMRV>
+cudaError_t launch_sweep_dense_grav(const SweepArgs& a, int nblocks, cudaStream_t st) {
+  static_assert(!AMRV || NDIM == 3, "the AMR variant is 3-D only");
+  constexpr int BX = 32, BY = tile_by_default(NDIM, RIEMANN);
+  constexpr size_t smem = sizeof(double) * SweepSmem<NDIM, BX, BY, true>::doubles;
+  auto kern = sweep_dense_kernel<NDIM, RIEMANN, -1, BX, BY, AMRV, false, true>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    configured = true;
+  }
+  kern<<<nblocks, dim3(BX, BY, 1), smem, st>>>(a);
+  return cudaGetLastError();
 }
 #endif
 
