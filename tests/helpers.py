@@ -47,13 +47,14 @@ class Case:
     """One run set-up: oracle mesh + params + the Fortran-side arrays (AmrCommons)."""
 
     def __init__(self, ndim, level, riemann="hllc", slope_type=1, bound=(0,) * 6, order=0, seed=1, boxlen=1.0,
-                 gamma=1.4, courant_factor=0.8, niter_riemann=10, slope_theta=1.5, nvector=32, nvar=None, coarse=(1, 1, 1)):
+                 gamma=1.4, courant_factor=0.8, niter_riemann=10, slope_theta=1.5, nvector=32, nvar=None, coarse=(1, 1, 1),
+                 smallr=1e-10, smallc=1e-10):
         """coarse = (nx, ny, nz) domain coarse cells; dx = boxlen / nx / 2^level"""
         self.ndim, self.level, self.nvar = ndim, level, (nvar or ndim + 2)      # nvar > ndim+2: passive scalars
         self.mesh = orc.Mesh(ndim, level, bound, order, seed, coarse=coarse)
         self.p = orc.make_params(ndim=ndim, nvar=self.nvar, riemann=riemann, slope_type=slope_type, boxlen=boxlen, gamma=gamma,
                                  courant_factor=courant_factor, niter_riemann=niter_riemann, slope_theta=slope_theta,
-                                 nvector=nvector)
+                                 nvector=nvector, smallr=smallr, smallc=smallc)
         self.riemann, self.slope_type = riemann, slope_type
         self.u = self.mesh.new_state(self.nvar)
 
@@ -227,6 +228,83 @@ def box_state(ndim, ext, seed=3, gamma=1.4):
         e = e + 0.5 * rho * vel[d] ** 2
     u[ndim + 1] = e
     return u
+
+
+# (smallr, smallc): the RAMSES defaults, and raised floors (smalle = smallc^2/gamma/(gamma-1) ~ 1.8e-4 at gamma = 1.4) that are
+# active across whole regions in the middle of the value range
+FLOORS = {"default": (1e-10, 1e-10), "raised": (1e-3, 1e-2)}
+
+
+def floor_state(ndim, ext, seed=1, smallr=1e-10, smallc=1e-10, gamma=1.4, nscalar=0):
+    """A hydro state that sits on the smallr / smalle floors, on a box of ext = (nx, ny, nz) cells (an int: a cube of ndim axes).
+    - density log-uniform per cell from 0.1 smallr to 1: jumps of many decades between neighbours, ~1/11 (default floors) to
+      ~1/4 (raised) of the cells below smallr;
+    - isolated near-vacuum cells (0.1-0.9 smallr) whose 2 ndim neighbours are dense and stream away from them, each with a random
+      transverse velocity: the predictor drives the face densities of those cells below smallr on all six faces;
+    - per-cell random velocities (random directions, speeds 0.1-3) and specific internal energies 1e-5-1;
+    - cold hypersonic cells, |v| = 10-100 sound speeds of a specific internal energy 1e-4-1e-2, with E = ekin (1 - delta),
+      delta in {0, 1e-14, 1e-3}: E/rho - ekin is zero or rounding-level or negative, so the internal-energy floor fires.
+    Returns the dense conservative array [ndim+2+nscalar][nz][ny][nx] (passive scalars rho*Z, Z in [0, 1])."""
+    if np.isscalar(ext):
+        ext = tuple(int(ext) if d < ndim else 1 for d in range(3))
+    shape = (ext[2], ext[1], ext[0])
+    rng = np.random.default_rng(seed)
+    rho = 10.0 ** rng.uniform(np.log10(0.1 * smallr), 0.0, shape)
+    eint = 10.0 ** rng.uniform(-5.0, 0.0, shape)
+    dirs = rng.standard_normal((ndim,) + shape)
+    vel = dirs * (10.0 ** rng.uniform(-1.0, 0.5, shape) / np.sqrt((dirs ** 2).sum(axis=0)))
+    vac = rng.random(shape) < 0.03
+    for d in range(ndim):
+        ax = 2 - d
+        for s in (-1, 1):
+            nb = np.roll(vac, s, axis=ax) & ~vac                 # the neighbour of a near-vacuum cell on side s of axis d
+            k = int(nb.sum())
+            rho[nb] = rng.uniform(0.5, 2.0, k)
+            for e in range(ndim):
+                vel[e][nb] = s * rng.uniform(1.0, 3.0, k) if e == d else rng.uniform(-1.0, 1.0, k)
+    rho[vac] = rng.uniform(0.1, 0.9, int(vac.sum())) * smallr
+    hyp = (rng.random(shape) < 0.08) & ~vac
+    k = int(hyp.sum())
+    rho[hyp] = 10.0 ** rng.uniform(np.log10(smallr), 0.0, k)
+    hdir = rng.standard_normal((ndim, k))
+    hdir /= np.sqrt((hdir ** 2).sum(axis=0))
+    c0 = np.sqrt(gamma * (gamma - 1) * 10.0 ** rng.uniform(-4.0, -2.0, k))
+    for e in range(ndim):
+        vel[e][hyp] = hdir[e] * c0 * rng.uniform(10.0, 100.0, k)
+    u = np.zeros((ndim + 2 + nscalar,) + shape)
+    u[0] = rho
+    ekin = np.zeros(shape)
+    for e in range(ndim):
+        u[1 + e] = rho * vel[e]
+        ekin = ekin + 0.5 * rho * vel[e] ** 2
+    u[ndim + 1] = rho * eint + ekin
+    u[ndim + 1][hyp] = ekin[hyp] * (1.0 - rng.choice([0.0, 1e-14, 1e-3], k))
+    for s in range(nscalar):
+        u[ndim + 2 + s] = rho * rng.random(shape)
+    return u
+
+
+def fill_floor_state(u, ndim, nvar, ncell, floors, seed):
+    """overwrite every cell of a tree state u (nvar x ncell, any shape of that size: active, boundary and parent cells alike)
+    with the cells of a floor_state under helpers.FLOORS[floors] and assert that the ctoprim floors fire on them; the tree's
+    cells are not neighbours in the floor_state, but its per-cell draws (densities down to 0.1 smallr, random velocities, cold
+    hypersonic cells) make every floor branch fire on a tree too.  Returns (smallr, smallc)."""
+    smallr, smallc = FLOORS[floors]
+    side = int(np.ceil(ncell ** (1.0 / ndim))) + 1
+    d = floor_state(ndim, side, seed, smallr, smallc, nscalar=nvar - ndim - 2).reshape(nvar, -1)[:, :ncell]
+    u.reshape(nvar, ncell)[:] = d
+    nrho, neint = floor_counts(d, ndim, smallr, smallc)
+    assert min(nrho, neint) >= 0.02 * ncell, (nrho, neint)
+    return smallr, smallc
+
+
+def floor_counts(u, ndim, smallr, smallc, gamma=1.4):
+    """(cells with rho < smallr, cells with E/max(rho, smallr) - ekin < smalle) of a dense conservative state: the cells on which
+    the density and internal-energy floors of ctoprim (hydro/umuscl.f90:894,923) fire"""
+    r = np.maximum(u[0], smallr)
+    ekin = sum(0.5 * (u[1 + d] / r) ** 2 for d in range(ndim))
+    smalle = smallc ** 2 / gamma / (gamma - 1)
+    return int((u[0] < smallr).sum()), int((u[ndim + 1] / r - ekin < smalle).sum())
 
 
 def level_slots(mesh, l, u, nvar):

@@ -10,6 +10,8 @@ import subprocess
 import numpy as np
 import pytest
 
+from helpers import FLOORS
+
 HERE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "host_numerics")
 CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "ramses_b200", "csrc")
 
@@ -47,6 +49,13 @@ def dev():
     L.devnum_mhd_amr_godunov.argtypes = [C.c_int] * 6 + [ip, ip, ip, ip, C.c_int, C.c_int, dp, dp, C.c_double, C.c_double] + [C.c_int] * 6 + \
         [C.c_double] * 3 + [C.c_int]
     L.devnum_mhd_amr_pass.argtypes = [C.c_int] * 7 + [ip, ip, ip, ip, C.c_int, dp] + [C.c_double] * 5 + [C.c_int, C.c_int, dp]
+    i3 = C.c_int * 3
+    L.devnum_sweep3_box.argtypes = [C.c_int, i3, i3, C.c_int, dp, dp] + [C.c_double] * 2 + [C.c_int] + [C.c_double] * 4 + \
+        [C.c_int, dp, C.c_int, C.c_int]
+    L.devnum_sweep_dense_box.argtypes = [C.c_int, C.c_int, i3, i3, C.c_int, dp, dp] + [C.c_double] * 2 + [C.c_int] + \
+        [C.c_double] * 4 + [C.c_int, dp, C.c_int]
+    L.devnum_sweep_dense_amr_box.argtypes = [C.c_int, i3, i3, C.c_int, dp, dp, C.POINTER(C.c_ubyte)] + [C.c_double] * 2 + \
+        [C.c_int] + [C.c_double] * 3 + [C.c_int]
     return L
 
 
@@ -65,6 +74,13 @@ def _hydro_states(rng, n, ndim):
     qr[k:2 * k, 0] = ql[k:2 * k, 0]
     ql[2 * k:2 * k + 50, 0] = 1e-12                                     # below smallr
     ql[2 * k + 50:2 * k + 100, 2] = 1e-30                               # below the pressure floor
+    ql[2 * k + 100:2 * k + 200, 2] = qr[2 * k + 100:2 * k + 200, 2] = 1e-30 # both sides at the pressure floor
+    ql[2 * k + 150:2 * k + 200, 0] = 1e-12                              # ... and at the density floor on one side
+    # strong rarefactions out of thin, cold gas: the star state of exact / acoustic has rstar < smallr and cstar < smallc
+    j, m = slice(2 * k + 200, 2 * k + 400), 200
+    ql[j, 0], qr[j, 0] = 10.0 ** rng.uniform(-8, -3, m), 10.0 ** rng.uniform(-8, -3, m)
+    ql[j, 2], qr[j, 2] = 10.0 ** rng.uniform(-16, -8, m), 10.0 ** rng.uniform(-16, -8, m)
+    ql[j, 1], qr[j, 1] = -(10.0 ** rng.uniform(-1, 2, m)), 10.0 ** rng.uniform(-1, 2, m)
     return np.ascontiguousarray(ql), np.ascontiguousarray(qr)
 
 
@@ -75,25 +91,50 @@ def test_hydro_riemann_device_formulas_equal_oracle(orc, dev, ndim, solver):
     bit for bit on 20 000 random face states -- including `exact`, whose only GPU-side deviation is CUDA's pow()."""
     n, nv = 20000, ndim + 2
     ql, qr = _hydro_states(np.random.default_rng(ndim * 10 + len(solver)), n, ndim)
-    fg = np.zeros((n, nv))
     sid = {"llf": 0, "exact": 1, "acoustic": 2, "hllc": 3, "hll": 4}[solver]
-    dev.devnum_riemann(ndim, sid, n, orc.dptr(ql), orc.dptr(qr), orc.dptr(fg), 1.4, 1e-10, 1e-10, 10)
-    p = orc.make_params(ndim=ndim, riemann=solver, nvector=n, niter_riemann=10)
     L = orc.lib()
     f = {"llf": L.orc_riemann_llf, "exact": L.orc_riemann_approx, "acoustic": L.orc_riemann_acoustic, "hllc": L.orc_riemann_hllc,
          "hll": L.orc_riemann_hll}[solver]
     f.argtypes = [C.POINTER(orc.Params), C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int]
-    qlf, qrf = np.asfortranarray(ql), np.asfortranarray(qr)              # (nvector, nvar) column-major
-    fgf = np.zeros((n, nv + 1), order="F")
-    f(C.byref(p), qlf.ctypes.data_as(C.POINTER(C.c_double)), qrf.ctypes.data_as(C.POINTER(C.c_double)),
-      fgf.ctypes.data_as(C.POINTER(C.c_double)), n)
-    assert np.isfinite(fg).all()
-    assert np.array_equal(fg, fgf[:, :nv])
-    # the internal-energy flux fgdnv(nvar+1) that only pressure_fix consumes (tmp2 of cmpflxm, umuscl.f90:848)
-    fe = np.zeros(n)
-    dev.devnum_riemann_eflux(ndim, sid, n, orc.dptr(ql), orc.dptr(qr), orc.dptr(fe), 1.4, 1e-10, 1e-10, 10)
-    assert np.isfinite(fe).all() and np.abs(fe).max() > 0
-    assert np.array_equal(fe, fgf[:, nv])
+    for smallr, smallc in FLOORS.values():
+        fg = np.zeros((n, nv))
+        dev.devnum_riemann(ndim, sid, n, orc.dptr(ql), orc.dptr(qr), orc.dptr(fg), 1.4, smallr, smallc, 10)
+        p = orc.make_params(ndim=ndim, riemann=solver, nvector=n, niter_riemann=10, smallr=smallr, smallc=smallc)
+        qlf, qrf = np.asfortranarray(ql), np.asfortranarray(qr)              # (nvector, nvar) column-major
+        fgf = np.zeros((n, nv + 1), order="F")
+        f(C.byref(p), qlf.ctypes.data_as(C.POINTER(C.c_double)), qrf.ctypes.data_as(C.POINTER(C.c_double)),
+          fgf.ctypes.data_as(C.POINTER(C.c_double)), n)
+        assert np.isfinite(fg).all()
+        assert np.array_equal(fg, fgf[:, :nv])
+        # the internal-energy flux fgdnv(nvar+1) that only pressure_fix consumes (tmp2 of cmpflxm, umuscl.f90:848)
+        fe = np.zeros(n)
+        dev.devnum_riemann_eflux(ndim, sid, n, orc.dptr(ql), orc.dptr(qr), orc.dptr(fe), 1.4, smallr, smallc, 10)
+        assert np.isfinite(fe).all() and np.abs(fe).max() > 0
+        assert np.array_equal(fe, fgf[:, nv])
+
+
+def _with_floor_cells(u, rng, ndim, k=400):
+    """u (n, ndim+2) conservative cells plus k cells on the floors of cmpdt (hydro/godunov_utils.f90:25,64) under both settings of
+    helpers.FLOORS: densities 1e-13-1e-4 (below smallr), and cold cells whose (gamma-1) e is below rho * smallp -- E = ekin (1 -
+    delta) with delta in {0, 1e-14, 1e-3}, or a specific internal energy of 1e-24-1e-5"""
+    nv = ndim + 2
+    f = np.zeros((2 * k, nv))
+    f[:, 0] = 10.0 ** rng.uniform(-4, 0, 2 * k)
+    f[:k, 0] = 10.0 ** rng.uniform(-13, -4, k)
+    vel = rng.standard_normal((2 * k, ndim)) * 10.0 ** rng.uniform(-2, 1, (2 * k, 1))
+    f[:, 1:1 + ndim] = f[:, :1] * vel
+    ekin = 0.5 * f[:, 0] * (vel ** 2).sum(axis=1)
+    f[:, nv - 1] = ekin + f[:, 0] * 10.0 ** rng.uniform(-5, 0, 2 * k)
+    f[k:, nv - 1] = np.where(rng.random(k) < 0.5, ekin[k:] * (1 - rng.choice([0.0, 1e-14, 1e-3], k)),
+                             ekin[k:] + f[k:, 0] * 10.0 ** rng.uniform(-24, -5, k))
+    return np.ascontiguousarray(np.concatenate([u, f]))
+
+
+def _assert_cmpdt_floors_fire(u, ndim, smallr, smallc, gamma=1.4):
+    r = np.maximum(u[:, 0], smallr)
+    e = u[:, ndim + 1] - 0.5 * r * sum((u[:, 1 + d] / r) ** 2 for d in range(ndim))
+    assert (u[:, 0] < smallr).sum() >= 100
+    assert ((gamma - 1) * e < r * smallc ** 2 / gamma).sum() >= 100
 
 
 @pytest.mark.parametrize("ndim", [1, 2, 3])
@@ -106,27 +147,32 @@ def test_hydro_cmpdt_with_gravity_device_formula_equals_oracle(orc, dev, ndim):
     vel = rng.standard_normal((n, ndim)) * 3
     u[:, 1:1 + ndim] = u[:, :1] * vel
     u[:, nv - 1] = 10.0 ** rng.uniform(-4, 2, n) + 0.5 * u[:, 0] * (vel ** 2).sum(axis=1)
+    u = _with_floor_cells(u, rng, ndim)
+    n = len(u)
     g = rng.standard_normal((n, ndim)) * 10.0 ** rng.uniform(-3, 5, (n, 1))
     g[:50] = 0.0
     dx = 1.0 / 128
     gsum = np.zeros(n)
     for d in range(ndim):                      # uu(k,1) = uu(k,1) + abs(gg(k,idim)) in this order
         gsum = gsum + np.abs(g[:, d])
-    dt = np.zeros(n)
-    dev.devnum_cmpdt_grav(ndim, n, orc.dptr(np.ascontiguousarray(u)), orc.dptr(gsum), dx, orc.dptr(dt), 1.4, 1e-10, 1e-10, 0.8)
-    p = orc.make_params(ndim=ndim, nvector=1, courant_factor=0.8)
     L = orc.lib()
     L.orc_cmpdt.argtypes = [C.POINTER(orc.Params), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_double, C.POINTER(C.c_double), C.c_int]
-    ref = np.zeros(n)
-    for i in range(n):
-        uu = u[i].copy()
-        gg = np.zeros(3)
-        gg[:ndim] = g[i]
-        o = C.c_double(0)
-        L.orc_cmpdt(C.byref(p), orc.dptr(uu), orc.dptr(gg), dx, C.byref(o), 1)
-        ref[i] = o.value
-    assert np.array_equal(dt, ref)
-    assert (dt[50:] < 0.999 * dt[:50].max()).any()
+    for smallr, smallc in FLOORS.values():
+        dt = np.zeros(n)
+        dev.devnum_cmpdt_grav(ndim, n, orc.dptr(np.ascontiguousarray(u)), orc.dptr(gsum), dx, orc.dptr(dt), 1.4, smallr, smallc, 0.8)
+        p = orc.make_params(ndim=ndim, nvector=1, courant_factor=0.8, smallr=smallr, smallc=smallc)
+        ref = np.zeros(n)
+        for i in range(n):
+            uu = u[i].copy()
+            gg = np.zeros(3)
+            gg[:ndim] = g[i]
+            o = C.c_double(0)
+            L.orc_cmpdt(C.byref(p), orc.dptr(uu), orc.dptr(gg), dx, C.byref(o), 1)
+            ref[i] = o.value
+        assert np.isfinite(ref).all()
+        assert np.array_equal(dt, ref)
+        assert (dt[50:] < 0.999 * dt[:50].max()).any()
+        _assert_cmpdt_floors_fire(u, ndim, smallr, smallc)
 
 
 @pytest.mark.parametrize("ndim", [1, 2, 3])
@@ -138,19 +184,24 @@ def test_hydro_cmpdt_device_formula_equals_oracle(orc, dev, ndim):
     vel = rng.standard_normal((n, ndim)) * 3
     u[:, 1:1 + ndim] = u[:, :1] * vel
     u[:, nv - 1] = 10.0 ** rng.uniform(-4, 2, n) + 0.5 * u[:, 0] * (vel ** 2).sum(axis=1)
-    dt = np.zeros(n)
+    u = _with_floor_cells(u, rng, ndim)
+    n = len(u)
     dx = 1.0 / 128
-    dev.devnum_cmpdt(ndim, n, orc.dptr(np.ascontiguousarray(u)), dx, orc.dptr(dt), 1.4, 1e-10, 1e-10, 0.8)
-    p = orc.make_params(ndim=ndim, nvector=1, courant_factor=0.8)
     L = orc.lib()
     L.orc_cmpdt.argtypes = [C.POINTER(orc.Params), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_double, C.POINTER(C.c_double), C.c_int]
-    ref = np.zeros(n)
-    for i in range(n):
-        uu = u[i].copy()
-        d = C.c_double(0.0)
-        L.orc_cmpdt(C.byref(p), orc.dptr(uu), None, dx, C.byref(d), 1)
-        ref[i] = d.value
-    assert np.array_equal(dt, ref)
+    for smallr, smallc in FLOORS.values():
+        dt = np.zeros(n)
+        dev.devnum_cmpdt(ndim, n, orc.dptr(np.ascontiguousarray(u)), dx, orc.dptr(dt), 1.4, smallr, smallc, 0.8)
+        p = orc.make_params(ndim=ndim, nvector=1, courant_factor=0.8, smallr=smallr, smallc=smallc)
+        ref = np.zeros(n)
+        for i in range(n):
+            uu = u[i].copy()
+            d = C.c_double(0.0)
+            L.orc_cmpdt(C.byref(p), orc.dptr(uu), None, dx, C.byref(d), 1)
+            ref[i] = d.value
+        assert np.isfinite(ref).all()
+        assert np.array_equal(dt, ref)
+        _assert_cmpdt_floors_fire(u, ndim, smallr, smallc)
 
 
 def _mhd_states(rng, n):
@@ -460,6 +511,34 @@ def test_amr_oct_batch_kernel_emulated_on_the_cpu_equals_oracle(orc, dev, ndim, 
     __shared__, a pthread barrier for __syncthreads) on an adaptively refined mesh: the update of the level's own cells equals
     godfine1 of the oracle (gather with prolongated ghost octs, unsplit, flux reset at refined faces, conservative update) bit
     for bit on every level.  The kernels that use warp shuffles / cp.async (the dense sweep) are outside this harness."""
+    _amr_oct_batch_compare(orc, dev, ndim, solver, difmag)
+
+
+@pytest.mark.parametrize("floors", ["default", "raised"])
+@pytest.mark.parametrize("ndim,solver,difmag", [(1, "hllc", 0.0), (2, "llf", 0.0), (2, "hllc", 0.1), (3, "hllc", 0.0), (3, "exact", 0.1)])
+def test_amr_oct_batch_kernel_emulated_at_the_floors(orc, dev, floors, ndim, solver, difmag):
+    """amr_godfine_kernel on the adaptively refined meshes of the test above with every cell holding a floor_state cell under the
+    RAMSES floors and raised ones: ctoprim's density and internal-energy floors and the face-density resets of the predictor
+    fire; the update of every level equals godfine1 of the oracle, bit for bit"""
+    _amr_oct_batch_compare(orc, dev, ndim, solver, difmag, floors)
+
+
+def _put_floor_state(r, ndim, floors, seed):
+    """a floor_state on every cell of the AMR run r (helpers.fill_floor_state) with the run's floors set to match; returns a time
+    step of Courant number ~0.3 on the finest level"""
+    from helpers import fill_floor_state
+    r.p.smallr, r.p.smallc = fill_floor_state(r.uold, ndim, ndim + 2, r.ncell, floors, seed)
+    d = r.uold.reshape(ndim + 2, r.ncell)
+    rho = np.maximum(d[0], r.p.smallr)
+    v2 = sum((d[1 + k] / rho) ** 2 for k in range(ndim))
+    eint = np.maximum(d[ndim + 1] / rho - 0.5 * v2, r.p.smallc ** 2 / 1.4 / 0.4)
+    vmax = float((np.sqrt(v2) + np.sqrt(1.4 * 0.4 * eint)).max())
+    return 0.3 * 0.5 ** r.nlevelmax * r.p.boxlen / vmax
+
+
+def _amr_oct_batch_compare(orc, dev, ndim, solver, difmag, floors=None):
+    """the body of test_amr_oct_batch_kernel_emulated_on_the_cpu_equals_oracle; floors: a floor_state on every cell instead of the
+    developed flow, under helpers.FLOORS[floors]"""
     from oracle.amr import FastAmrRun
     if ndim == 1:
         reg = [dict(type="square", x_center=0.25, length_x=0.5, d=1.0, p=1.0), dict(type="square", x_center=0.75, length_x=0.5, d=0.125, p=0.1)]
@@ -479,6 +558,7 @@ def test_amr_oct_batch_kernel_emulated_on_the_cpu_equals_oracle(orc, dev, ndim, 
                        interpol_type=1, regions=reg, tout=[1e9])
         itype, st = 1, 1
     r.run(max_coarse=3)
+    dt_floor = _put_floor_state(r, ndim, floors, 40 + ndim) if floors else None
     r.p.difmag = difmag                                  # artificial diffusion (cmpdivu / consup) for the comparison step only
     m = r.m
     T, nvar = 1 << ndim, ndim + 2
@@ -493,6 +573,8 @@ def test_amr_oct_batch_kernel_emulated_on_the_cpu_equals_oracle(orc, dev, ndim, 
         if len(act) == 0:
             continue
         dt = 0.4 * r.dtnew[r.levelmin] / 2 ** (l - r.levelmin) if r.dtnew[r.levelmin] > 0 else 1e-4
+        if floors:
+            dt = dt_floor * 2 ** (r.nlevelmax - l)
         dx = 0.5 ** l * r.p.boxlen / (m.icoarse_max - m.icoarse_min + 1)
         # oracle: set_unew + godunov_fine of this level only
         unew_o = np.zeros_like(r.uold)
@@ -504,7 +586,8 @@ def test_amr_oct_batch_kernel_emulated_on_the_cpu_equals_oracle(orc, dev, ndim, 
         rflux = np.zeros(len(act) * 2 * ndim * (T // 2) * nvar)
         dev.devnum_amr_godfine(ndim, sid, r.ncoarse, r.ngridmax, m.nx, m.ny, m.nz, orc.iptr(son), orc.iptr(father), orc.iptr(nbor),
                                orc.iptr(act), len(act), l, orc.dptr(r.uold), orc.dptr(unew_k), orc.dptr(rflux), dt, dx, itype, st,
-                               1.4, 1e-10, 1e-10, 10, difmag)
+                               1.4, r.p.smallr, r.p.smallc, 10, difmag)
+        assert np.isfinite(unew_o).all()
         Uo, Uk = unew_o.reshape(nvar, r.ncell), unew_k.reshape(nvar, r.ncell)
         for ind in range(T):
             c = r.ncoarse + ind * r.ngridmax + act.astype(np.int64) - 1
@@ -523,6 +606,23 @@ def test_amr_source_terms_emulated_on_the_cpu_equal_oracle(orc, dev, ndim, solve
     emulated launch, and the list passes of set_unew / set_uold (divu/enew reset, add_gravity_source_terms,
     add_pdv_source_terms, the energy switch) equal the oracle's set_unew -> godunov_fine -> set_uold bit for bit on the level's
     own cells (state, divu and enew)."""
+    _amr_source_terms_compare(orc, dev, ndim, solver, grav, pfix)
+
+
+@pytest.mark.parametrize("floors", ["default", "raised"])
+@pytest.mark.parametrize("ndim,solver,grav,pfix", [(1, "hllc", True, True), (2, "exact", False, True), (2, "llf", True, False),
+                                                    (3, "hllc", True, True), (3, "acoustic", False, True)])
+def test_amr_source_terms_emulated_at_the_floors(orc, dev, floors, ndim, solver, grav, pfix):
+    """poisson and pressure_fix on the refined meshes of the test above with every cell holding a floor_state cell: the gravity
+    predictor and add_gravity_source_terms on floored densities (d_old = max(uold, smallr), godunov_fine.f90:267), enew / divu
+    and add_pdv_source_terms at cold hypersonic cells, and the energy switch, which fires there on every level -- equal the
+    oracle's set_unew -> godunov_fine -> set_uold bit for bit"""
+    _amr_source_terms_compare(orc, dev, ndim, solver, grav, pfix, floors)
+
+
+def _amr_source_terms_compare(orc, dev, ndim, solver, grav, pfix, floors=None):
+    """the body of test_amr_source_terms_emulated_on_the_cpu_equal_oracle; floors: a floor_state on every cell, under
+    helpers.FLOORS[floors]"""
     from oracle.amr import FastAmrRun
     if ndim == 1:
         reg = [dict(type="square", x_center=0.25, length_x=0.5, d=1.0, p=1.0), dict(type="square", x_center=0.75, length_x=0.5, d=0.125, p=0.1)]
@@ -542,6 +642,7 @@ def test_amr_source_terms_emulated_on_the_cpu_equal_oracle(orc, dev, ndim, solve
                        interpol_type=1, regions=reg, tout=[1e9])
         itype, st = 1, 1
     r.run(max_coarse=3)
+    dt_floor = _put_floor_state(r, ndim, floors, 50 + ndim) if floors else None
     m = r.m
     T, nvar, nc = 1 << ndim, ndim + 2, r.ncell
     son = np.ascontiguousarray(r.son[1:], dtype=np.int32)
@@ -562,6 +663,8 @@ def test_amr_source_terms_emulated_on_the_cpu_equal_oracle(orc, dev, ndim, solve
             if len(act) == 0:
                 continue
             dt = 0.4 * r.dtnew[r.levelmin] / 2 ** (l - r.levelmin) if r.dtnew[r.levelmin] > 0 else 1e-4
+            if floors:
+                dt = dt_floor * 2 ** (r.nlevelmax - l)
             dx = 0.5 ** l * r.p.boxlen / (m.icoarse_max - m.icoarse_min + 1)
             cells = np.concatenate([r.ncoarse + ind * r.ngridmax + act.astype(np.int64) - 1 for ind in range(T)])
             # ---- oracle: set_unew -> godunov_fine -> set_uold of this level with the options on
@@ -585,13 +688,13 @@ def test_amr_source_terms_emulated_on_the_cpu_equal_oracle(orc, dev, ndim, solve
             if pfix:
                 divu_k[:] = 7.0; enew_k[:] = -3.0
             args = (ndim, r.ncoarse, r.ngridmax, m.nx, m.ny, m.nz, orc.iptr(son), orc.iptr(father), orc.iptr(nbor), orc.iptr(act), len(act))
-            tail = (orc.dptr(force), 1.4, 1e-10, beta_fix, dx, dt)
+            tail = (orc.dptr(force), 1.4, r.p.smallr, beta_fix, dx, dt)
             if pfix:
                 dev.devnum_amr_src_pass(0, *args, orc.dptr(uold_k), orc.dptr(unew_k), orc.dptr(divu_k), orc.dptr(enew_k), *tail)
             rflux = np.zeros(len(act) * 2 * ndim * (T // 2) * ncol)
             dev.devnum_amr_godfine_src(ndim, sid, r.ncoarse, r.ngridmax, m.nx, m.ny, m.nz, orc.iptr(son), orc.iptr(father), orc.iptr(nbor),
                                        orc.iptr(act), len(act), l, orc.dptr(uold_k), orc.dptr(unew_k), orc.dptr(rflux), dt, dx, itype, st,
-                                       1.4, 1e-10, 1e-10, 10, orc.dptr(force) if grav else None, 1 if pfix else 0, r.nvector)
+                                       1.4, r.p.smallr, r.p.smallc, 10, orc.dptr(force) if grav else None, 1 if pfix else 0, r.nvector)
             # after the sweep and the coarse reflux pass, before the sources: the WHOLE arrays -- the level's own cells and the coarser
             # cells that received refluxes (state, and with pressure_fix divu / enew, which reflux like two more variables)
             assert np.array_equal(unew_k[: nvar * nc], unew_mid), l
@@ -619,8 +722,9 @@ def test_amr_source_terms_emulated_on_the_cpu_equal_oracle(orc, dev, ndim, solve
         L.orc_set_pressure_fix(None, None, 0.0)
         L.orc_set_gravity(None)
     assert nlev >= 3 and gmoved > 1e-6 and (dmax > 0 or not pfix) and nrefl > 0
-    if pfix and ndim == 3:
-        assert switched > 0          # the cold Sedov background (p = 1e-5) does trip the energy switch
+    if pfix and (ndim == 3 or floors):
+        assert switched > 0          # the cold Sedov background (p = 1e-5) and the cold hypersonic cells trip the energy switch
+    assert np.isfinite(uold_o).all()
 
 
 MHD_R1D = {"llf": 0, "roe": 1, "hll": 2, "hlld": 3, "upwind": 4, "hydro": 5}
@@ -1003,12 +1107,13 @@ def test_vec_solvers_equal_scalar(orc, dev, solver):
     ql[100:200, 1] = 50.0; qr[100:200, 1] = 50.0
     ql[200:300, 1] = -50.0; qr[200:300, 1] = -50.0
     sid = {"llf": 0, "exact": 1, "acoustic": 2, "hllc": 3, "hll": 4}[solver]
-    ref, f1, f3 = np.zeros((n, 5)), np.zeros((n, 5)), np.zeros((n, 5))
-    dev.devnum_riemann(3, sid, n, orc.dptr(ql), orc.dptr(qr), orc.dptr(ref), 1.4, 1e-10, 1e-10, 10)
-    dev.devnum_riemann_vec(sid, n, orc.dptr(ql), orc.dptr(qr), orc.dptr(f1), orc.dptr(f3), 1.4, 1e-10, 1e-10, 10)
-    assert np.isfinite(ref).all()
-    assert np.array_equal(f1, ref)
-    assert np.array_equal(f3, ref)
+    for smallr, smallc in FLOORS.values():
+        ref, f1, f3 = np.zeros((n, 5)), np.zeros((n, 5)), np.zeros((n, 5))
+        dev.devnum_riemann(3, sid, n, orc.dptr(ql), orc.dptr(qr), orc.dptr(ref), 1.4, smallr, smallc, 10)
+        dev.devnum_riemann_vec(sid, n, orc.dptr(ql), orc.dptr(qr), orc.dptr(f1), orc.dptr(f3), 1.4, smallr, smallc, 10)
+        assert np.isfinite(ref).all()
+        assert np.array_equal(f1, ref)
+        assert np.array_equal(f3, ref)
 
 
 @pytest.mark.parametrize("solver,st,N,nblocks,by,vec", [("hllc", 1, 16, 3, 12, 1), ("hllc", 2, 16, 2, 12, 0), ("hllc", 1, 16, 5, 12, 2),
@@ -1229,14 +1334,21 @@ def test_dense_sweep_amr_variant_emulated_on_non_cubic_boxes(orc, dev, coarse, b
     """sweep_dense_kernel<..., AMRV=true> on a 48x32x16 periodic base level and on a 16x32x48 base level between outflow x ends, a
     scattered tenth of its cells marked refined (son > 0): fluxes through refined faces reset, the update accumulated into a unew
     that already holds the finer level's refluxes -- equals set_unew + godunov_fine of the oracle on that level, bit for bit"""
-    from helpers import Case, box_state, level_slots
+    _dense_amr_box_compare(orc, dev, coarse, bound, solver, nblocks)
+
+
+def _dense_amr_box_compare(orc, dev, coarse, bound, solver, nblocks, floors=None):
+    """the body of the test above; floors = a key of helpers.FLOORS: a floor_state under those floors in place of the box_state"""
+    from helpers import FLOORS, Case, box_state, floor_state, level_slots
+    smallr, smallc = FLOORS[floors] if floors else (1e-10, 1e-10)
     dev.devnum_sweep_dense_amr_box.argtypes = [C.c_int, IP3, IP3, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double),
                                                C.POINTER(C.c_ubyte), C.c_double, C.c_double, C.c_int, C.c_double, C.c_double,
                                                C.c_double, C.c_int]
     lev = 4
-    c = Case(3, lev, riemann=solver, slope_type=1, bound=bound, coarse=coarse, boxlen=float(coarse[0]), order=2, seed=8)
+    c = Case(3, lev, riemann=solver, slope_type=1, bound=bound, coarse=coarse, boxlen=float(coarse[0]), order=2, seed=8,
+             smallr=smallr, smallc=smallc)
     ext = c.mesh.extent(lev)
-    c.init_dense(box_state(3, ext))
+    c.init_dense(floor_state(3, ext, 8, smallr, smallc) if floors else box_state(3, ext))
     s = c.mesh.s
     act = c.mesh.active(lev).astype(np.int64)
     cells = np.concatenate([s.ncoarse + ind * s.ngridmax + act for ind in range(8)])        # 1-based
@@ -1265,8 +1377,9 @@ def test_dense_sweep_amr_variant_emulated_on_non_cubic_boxes(orc, dev, coarse, b
     unmasked = uout.copy()
     for mask, out in ((refined, uout), (np.zeros_like(refined), unmasked)):
         dev.devnum_sweep_dense_amr_box(SOLVER_ID[solver], IP3(*ext), IP3(*shell), nblocks, orc.dptr(uin), orc.dptr(out),
-                                       mask.ctypes.data_as(C.POINTER(C.c_ubyte)), dt, 2.0 ** -lev, 1, 1.4, 1e-10, 1e-10, 10)
+                                       mask.ctypes.data_as(C.POINTER(C.c_ubyte)), dt, 2.0 ** -lev, 1, 1.4, smallr, smallc, 10)
     assert not np.array_equal(unmasked, uout)              # the marks matter
+    assert np.isfinite(unew).all()
     Un, Us = unew.reshape(5, s.ncell), start.reshape(5, s.ncell)
     moved = 0.0
     for ind in range(8):
@@ -1274,3 +1387,78 @@ def test_dense_sweep_amr_variant_emulated_on_non_cubic_boxes(orc, dev, coarse, b
         moved = max(moved, np.abs(Un[:, cc] - Us[:, cc]).max())
         assert np.array_equal(uout[:, ind, slot], Un[:, cc]), (ind, float(np.abs(uout[:, ind, slot] - Un[:, cc]).max()))
     assert moved > 1e-5
+
+
+# ---- the floors: near-vacuum and cold hypersonic states on which smallr / smalle fire (helpers.floor_state) ----
+def _floor_case(ndim, ext, solver, st, floors, seed, bound=(0,) * 6):
+    """oracle level step on a floor_state of ext cells (one coarse cell per 16 cells in x: dx = 1/16) under the floors
+    helpers.FLOORS[floors]; asserts the state makes the ctoprim floors fire and the oracle stays finite"""
+    from helpers import FLOORS, Case, floor_counts, floor_state
+    smallr, smallc = FLOORS[floors]
+    level = 4 if ext[0] >= 16 else int(np.log2(ext[0]))
+    coarse = tuple(max(e >> level, 1) for e in ext)
+    c = Case(ndim, level, riemann=solver, slope_type=st, slope_theta=1.3, bound=bound, coarse=coarse, boxlen=float(coarse[0]),
+             order=1, seed=2, smallr=smallr, smallc=smallc)
+    assert tuple(c.mesh.extent(level))[:ndim] == tuple(ext)[:ndim]
+    d0 = floor_state(ndim, c.mesh.extent(level), seed, smallr, smallc)
+    nrho, neint = floor_counts(d0, ndim, smallr, smallc)
+    ncell = d0[0].size
+    assert min(nrho, neint) >= max(2, 0.02 * ncell), (nrho, neint)
+    c.init_dense(d0)
+    dt, _ = c.oracle_courant()
+    unew = c.oracle_godunov(dt, nthreads=1)
+    assert np.isfinite(dt) and dt > 0 and np.isfinite(unew).all()
+    return c, c.mesh.extent(level), dt, unew
+
+
+@pytest.mark.parametrize("floors", ["default", "raised"])
+@pytest.mark.parametrize("solver,st,nblocks,by,vec", [("llf", 1, 3, 12, 1), ("exact", 2, 2, 12, 1), ("acoustic", 8, 3, 12, 1),
+                                                      ("hllc", 1, 5, 12, 0), ("hll", 2, 3, 16, 2), ("hllc", 8, 3, 12, 12),
+                                                      ("exact", 1, 4, 12, 40), ("hllc", 2, 5, 12, 41), ("llf", 8, 3, 12, 42),
+                                                      ("hll", 1, 4, 8, 41)])
+def test_sweep3_kernel_emulated_at_the_floors(orc, dev, floors, solver, st, nblocks, by, vec):
+    """sweep3_kernel (solver forms 0 / 1 / 2, the 12 form) and sweep4_kernel (40-42) on a 16^3 floor_state: near-vacuum cells
+    whose six face densities the predictor drives below smallr (the y face passing through shared memory), densities below
+    smallr and cold hypersonic cells with E/rho - ekin below smalle, under the RAMSES floors and raised ones -- the new state and
+    the fused Courant partials equal the oracle's, bit for bit"""
+    from helpers import level_slots
+    c, ext, dt, unew = _floor_case(3, (16, 16, 16), solver, st, floors, 11 + vec)
+    uin, act, slot = level_slots(c.mesh, c.level, c.u, 5)
+    uout = np.zeros_like(uin)
+    part = np.zeros(4 * 64)
+    nb = dev.devnum_sweep3_box(SOLVER_ID[solver], IP3(*ext), IP3(0, 0, 0), nblocks, orc.dptr(uin), orc.dptr(uout), dt,
+                               2.0 ** -c.level, st, 1.3, 1.4, c.p.smallr, c.p.smallc, 10, orc.dptr(part), by, vec)
+    _check_box_result(c, uout, act, slot, unew, part, nb, 3)
+
+
+@pytest.mark.parametrize("floors", ["default", "raised"])
+@pytest.mark.parametrize("ndim,ext,bound,solver,st,nblocks", [
+    (1, (64, 1, 1), (0,) * 6, "hllc", 2, 2),
+    (1, (64, 1, 1), (1, 1, 0, 0, 0, 0), "exact", 1, 1),
+    (2, (32, 32, 1), (0,) * 6, "llf", 8, 3),
+    (2, (32, 32, 1), (0, 0, 2, 2, 0, 0), "acoustic", 1, 2),
+    (3, (16, 16, 16), (0,) * 6, "hll", 2, 3),
+    (3, (16, 16, 16), (0,) * 6, "exact", 8, 4),
+    (3, (16, 16, 16), (1, 1, 0, 0, 0, 0), "hllc", 1, 5),
+])
+def test_dense_sweep_kernel_emulated_at_the_floors(orc, dev, floors, ndim, ext, bound, solver, st, nblocks):
+    """sweep_dense_kernel (1-D, 2-D and 3-D forms) on a floor_state, periodic or with a wall / outflow shell: ctoprim's density and
+    internal-energy floors and the face-density resets of the predictor fire; the owned cells and the fused Courant partials
+    equal the oracle's, bit for bit"""
+    from helpers import level_slots
+    c, ext, dt, unew = _floor_case(ndim, ext, solver, st, floors, 5 + nblocks, bound=bound)
+    shell = [int(bound[2 * d] > 0) for d in range(3)]
+    uin, act, slot = level_slots(c.mesh, c.level, c.u, ndim + 2)
+    uout = np.zeros_like(uin)
+    part = np.zeros(4 * 64)
+    nb = dev.devnum_sweep_dense_box(ndim, SOLVER_ID[solver], IP3(*ext), IP3(*shell), nblocks, orc.dptr(uin), orc.dptr(uout), dt,
+                                    2.0 ** -c.level, st, 1.3, 1.4, c.p.smallr, c.p.smallc, 10, orc.dptr(part), 0)
+    _check_box_result(c, uout, act, slot, unew, part, nb, ndim)
+
+
+@pytest.mark.parametrize("floors", ["default", "raised"])
+@pytest.mark.parametrize("solver", ["hllc", "exact"])
+def test_dense_sweep_amr_variant_emulated_at_the_floors(orc, dev, floors, solver):
+    """sweep_dense_kernel<..., AMRV=true> on a 48x32x16 base level holding a floor_state, a tenth of its cells marked refined:
+    equals set_unew + godunov_fine of the oracle, bit for bit"""
+    _dense_amr_box_compare(orc, dev, (3, 2, 1), (0,) * 6, solver, 5, floors=floors)

@@ -27,6 +27,7 @@ def commons_from_run(r, riemann, slope_type):
     a.gamma, a.courant_factor = r.p.gamma, r.p.courant_factor
     a.slope_type, a.riemann, a.nvector = slope_type, riemann, r.nvector
     a.difmag = r.p.difmag
+    a.smallr, a.smallc = r.p.smallr, r.p.smallc
     return a
 
 
@@ -70,7 +71,10 @@ BOUND_2D_WALLS_X_OUTFLOW_Y = [(1, (0, 0), (1, 1), (0, 0)), (2, (2, 2), (1, 1), (
 
 def run_case(ndim, levelmin, levelmax, bound, regions, riemann, slope_type, ncoarse_dev, interpol_type, nsub, boxlen=1.0,
              err=0.05, nexpand=1, difmag=0.0, bound_regions=None, interpol_var=0, gravity=False, pressure_fix=False, beta_fix=0.5,
-             device_resident=False):
+             device_resident=False, floors=None):
+    """one coarse step of an adaptively refined mesh, developed by the oracle's regridding driver and then frozen, on the GPU
+    (host-driven amr_step order, or rgpu_amr_steps) and on the oracle; floors: every cell then holds a floor_state cell under
+    helpers.FLOORS[floors] (helpers.fill_floor_state) for the compared step"""
     from oracle.amr import AmrRun
     from ramses_b200.hydro import HydroGPU
     r = AmrRun(ndim, levelmin, levelmax, bound, boxlen, nsubcycle=nsub, nexpand=nexpand, ngridmax=20000, riemann=riemann,
@@ -98,6 +102,9 @@ def run_case(ndim, levelmin, levelmax, bound, regions, riemann, slope_type, ncoa
         r.refine_fine(i)
     nlev = [len(r.active[l]) for l in range(1, levelmax + 1)]
     assert sum(1 for n in nlev[levelmin:] if n > 0) >= 1, nlev      # a genuinely refined mesh
+    if floors:
+        from helpers import fill_floor_state
+        r.p.smallr, r.p.smallc = fill_floor_state(r.uold, ndim, r.nvar, m_ncell(r), floors, 60 + ndim)
     a = commons_from_run(r, riemann, slope_type)
     # source terms are switched on for the compared coarse step only (the mesh was developed without them): poisson with an
     # arbitrary acceleration field f (an INPUT of the path) and pressure_fix (divu / enew, reset by set_unew of every level)

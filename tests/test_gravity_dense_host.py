@@ -181,3 +181,43 @@ def test_gravity_dense_sweep_amr_variant_emulated_equals_oracle(orc, grav_dev, c
     for ind in range(8):
         cc = s.ncoarse + ind * s.ngridmax + act - 1
         assert np.array_equal(uout[:, ind, slot], Un[:, cc]), (ind, float(np.abs(uout[:, ind, slot] - Un[:, cc]).max()))
+
+
+@pytest.mark.parametrize("floors", ["default", "raised"])
+@pytest.mark.parametrize("ndim,ext,solver,st,nblocks", [(1, (64, 1, 1), "hllc", 2, 2), (2, (32, 32, 1), "exact", 1, 3),
+                                                       (3, (16, 16, 16), "llf", 8, 4), (3, (16, 16, 16), "hllc", 1, 3)])
+def test_gravity_dense_sweep_emulated_at_the_floors(orc, grav_dev, floors, ndim, ext, solver, st, nblocks):
+    """sweep_dense_kernel<..., GRAV> with the fused source term on a floor_state (densities below smallr, cold hypersonic cells,
+    near-vacuum cells streamed out of) under the RAMSES floors and raised ones, with an acceleration strong enough that the
+    predictor moves floored face densities: ctoprim's floors, the face resets after the gravity predictor and
+    add_gravity_source_terms' d_old = max(uold, smallr) (hydro/godunov_fine.f90:267) all fire; the owned cells and the next dt
+    equal the oracle's with the same f, bit for bit"""
+    from helpers import FLOORS, Case, floor_counts, floor_state, level_slots
+    smallr, smallc = FLOORS[floors]
+    level = 4 if ndim == 3 else 5
+    coarse = tuple(max(e >> level, 1) for e in ext)
+    c = Case(ndim, level, riemann=solver, slope_type=st, slope_theta=1.3, coarse=coarse, boxlen=float(coarse[0]), order=1, seed=2,
+             smallr=smallr, smallc=smallc)
+    d0 = floor_state(ndim, c.mesh.extent(level), 31 + ndim, smallr, smallc)
+    nrho, neint = floor_counts(d0, ndim, smallr, smallc)
+    assert min(nrho, neint) >= max(2, 0.02 * d0[0].size), (nrho, neint)
+    c.init_dense(d0)
+    s = c.mesh.s
+    f = force_field(ndim, s.ncell, 200.0, 17 + ndim)
+    dt, unew = _oracle_level_step(c, f, 1)
+    with Gravity(f):
+        dt_next, sums = c.oracle_courant(unew)
+    assert np.isfinite(unew).all() and np.isfinite(dt_next)
+    uin, act, slot = level_slots(c.mesh, level, c.u, ndim + 2)
+    fin, _, _ = level_slots(c.mesh, level, f.ravel(), ndim)
+    uout = np.zeros_like(uin)
+    part = np.zeros(4 * 64)
+    nb = grav_dev.devnum_sweep_dense_grav_box(ndim, SOLVER_ID[solver], IP3(*c.mesh.extent(level)), IP3(0, 0, 0), nblocks, orc.dptr(uin),
+                                              orc.dptr(uout), orc.dptr(fin), 1, None, dt, 2.0 ** -level, st, 1.3, 1.4, smallr, smallc, 10,
+                                              orc.dptr(part))
+    U = unew.reshape(ndim + 2, s.ncell)
+    for ind in range(1 << ndim):
+        cells = s.ncoarse + ind * s.ngridmax + act - 1
+        assert np.array_equal(uout[:, ind, slot], U[:, cells]), (ind, float(np.abs(uout[:, ind, slot] - U[:, cells]).max()))
+    p4 = part[:4 * nb].reshape(4, nb)
+    assert min(p4[0].min(), c.p.boxlen / c.p.smallc) == dt_next
