@@ -21,13 +21,15 @@ NV, NVS = 8, 11
 class MhdAmrRun(AmrRun):
     def __init__(self, levelmin, levelmax, bound_type, boxlen, nsubcycle, riemann="hlld", slope_type=1, gamma=1.4,
                  courant_factor=0.8, err_grad_d=-1.0, err_grad_u=-1.0, err_grad_p=-1.0, err_grad_A=-1.0, err_grad_B=-1.0,
-                 err_grad_C=-1.0, err_grad_B2=-1.0, interpol_type=1, regions=(), tout=(), nexpand=1, ngridmax=2000, nvector=32):
+                 err_grad_C=-1.0, err_grad_B2=-1.0, interpol_type=1, regions=(), tout=(), nexpand=1, ngridmax=2000, nvector=32,
+                 smallr=1e-10, smallc=1e-10):
         super().__init__(1, levelmin, levelmax, bound_type, boxlen, nsubcycle, nexpand=nexpand, ngridmax=ngridmax,
                          riemann="llf", slope_type=slope_type, gamma=gamma, courant_factor=courant_factor,
                          err_grad_d=err_grad_d, err_grad_u=err_grad_u, err_grad_p=err_grad_p, interpol_type=interpol_type,
                          interpol_var=0, regions=regions, tout=tout, nvector=nvector)
         self.pm = orc.make_mhd_params(slope_type=slope_type, riemann=riemann, riemann2d="llf", gamma=gamma,
-                                      courant_factor=courant_factor, boxlen=boxlen)
+                                      courant_factor=courant_factor, boxlen=boxlen, smallr=smallr, smallc=smallc)
+        self.p.smallr, self.p.smallc = smallr, smallc      # the driver's own floors (dtnew = boxlen / smallc, region fill)
         self.nvar = NVS                                   # stored variables (nvar+3 of the MHD build)
         self.uold = np.zeros(NVS * self.ncell)
         self.unew = np.zeros(NVS * self.ncell)
@@ -233,13 +235,14 @@ class MhdAmrRun2D(FastAmrRun):
     def __init__(self, levelmin, levelmax, boxlen, nsubcycle, riemann="hlld", riemann2d="hlld", slope_type=2, gamma=1.4,
                  courant_factor=0.8, err_grad_d=-1.0, err_grad_u=-1.0, err_grad_p=-1.0, err_grad_A=-1.0, err_grad_B=-1.0,
                  err_grad_C=-1.0, err_grad_B2=-1.0, interpol_type=2, tout=(), nexpand=1, ngridmax=100000, nvector=32,
-                 ic="orszag_tang", nthreads=None):
+                 ic="orszag_tang", nthreads=None, smallr=1e-10, smallc=1e-10):
         super().__init__(self.NDIM, levelmin, levelmax, (0, 0, 0, 0, 0, 0), boxlen, nsubcycle, nexpand=nexpand, ngridmax=ngridmax,
                          riemann="llf", slope_type=slope_type, gamma=gamma, courant_factor=courant_factor,
                          err_grad_d=err_grad_d, err_grad_u=err_grad_u, err_grad_p=err_grad_p, interpol_type=interpol_type,
                          interpol_var=0, regions=(), tout=tout, nvector=nvector, nthreads=nthreads)
         self.pm = orc.make_mhd_params(slope_type=slope_type, riemann=riemann, riemann2d=riemann2d, gamma=gamma,
-                                      courant_factor=courant_factor, boxlen=boxlen)
+                                      courant_factor=courant_factor, boxlen=boxlen, smallr=smallr, smallc=smallc)
+        self.p.smallr, self.p.smallc = smallr, smallc
         self.nvar = NVS
         self.uold = np.zeros(NVS * self.ncell)
         self.unew = np.zeros(NVS * self.ncell)

@@ -307,6 +307,157 @@ def floor_counts(u, ndim, smallr, smallc, gamma=1.4):
     return int((u[0] < smallr).sum()), int((u[ndim + 1] / r - ekin < smalle).sum())
 
 
+def mhd_floor_state(ext, seed=1, smallr=1e-10, smallc=1e-10, gamma=5.0 / 3.0, slab_vt=0.0):
+    """An ideal-MHD state that sits on the smallr / pressure floors and where the field degenerates, on a periodic box of
+    ext = (nx, ny, nz) cells (h = 1/nx, every axis >= 8).  The staggered field is the curl of an edge potential plus per-axis
+    uniform parts that do not depend on the coordinate along their own axis: divergence-free to round-off, and both copies of
+    every shared face (the periodic wrap included) hold the same number.  Regions:
+    - field-free sub-box (x < nx/2, y >= ny/2, z >= nz/2): the potential is zero on every edge of its cells and no uniform part
+      crosses it, so B = 0 exactly on all its faces;
+    - field-aligned slab (y < ny/4, z < nz/4, all x): B = (bx(y,z), 0, 0) exactly, v = (vx, slab_vt vy, slab_vt vz) (slab_vt = 0:
+      the 1-D solvers see exactly aligned states; the 2-D hlla solver needs slab_vt > 0, because its corner EMF is 0/0, in the
+      reference too, when all four corners have zero transverse velocity and field), pressure set so that
+      vA^2 / c_s^2 is 2-20 in half of its cells and 0.05-0.5 in the other half (never 1: there the fast speed of an
+      axis-aligned field is the square root of a rounding residue, in the reference too);
+    - elsewhere the potential's amplitude changes per 4^3 block over 1e-12-1, so fields from 1e-12 to O(1) meet;
+    - densities log-uniform from 0.1 smallr to 1 and isolated near-vacuum cells whose neighbours stream away (floor_state);
+    - cold magnetised cells E = ekin + emag (1 - delta) and cold hypersonic cells E = ekin (1 - delta) + emag, delta in
+      {0, 1e-14, 1e-3}: the raw pressure is zero, rounding-level or negative;
+    - magnetically dominated near-vacuum cells, plasma beta 1e-20-1e-6.
+    Returns the dense conservative array [11][nz][ny][nx]."""
+    nx, ny, nz = ext
+    assert min(ext) >= 8
+    h = 1.0 / nx
+    shape = (nz, ny, nx)
+    rng = np.random.default_rng(seed)
+    Z, Y, X = np.meshgrid(np.arange(nz), np.arange(ny), np.arange(nx), indexing="ij")
+    free = (X < nx // 2) & (Y >= ny // 2) & (Z >= nz // 2)
+    slab = (Y < ny // 4) & (Z < nz // 4)
+    quiet = free | slab
+    dn = lambda a, ax: np.roll(a, 1, axis=ax)                  # value of the lower neighbour
+    up = lambda a, ax: np.roll(a, -1, axis=ax)
+    # edge potential (low edges of every cell), zero on every edge of a quiet cell
+    scale = 10.0 ** rng.choice([-12.0, -6.0, -2.0, -0.5, 0.0], (nz // 4 + 1, ny // 4 + 1, nx // 4 + 1))[Z // 4, Y // 4, X // 4]
+    pot = []
+    for a0, a1 in ((0, 1), (0, 2), (1, 2)):                    # Ax touches cells shifted in z,y; Ay in z,x; Az in y,x
+        touch = quiet | dn(quiet, a0) | dn(quiet, a1) | dn(dn(quiet, a0), a1)
+        pot.append(np.where(touch, 0.0, h * scale * rng.standard_normal(shape)))
+    Ax, Ay, Az = pot
+    # uniform parts: Bx(y,z), By(x,z), Bz(x,y), zero on every line through a quiet cell; the slab's own bx(y,z)
+    gx = np.where(quiet.any(axis=2, keepdims=True), 0.0, 0.4) * np.ones(shape)
+    gy = np.where(quiet.any(axis=1, keepdims=True), 0.0, -0.3) * np.ones(shape)
+    gz = np.where(quiet.any(axis=0, keepdims=True), 0.0, 0.25) * np.ones(shape)
+    fs = rng.uniform(0.2, 1.0, (nz, ny, 1)) * rng.choice([-1.0, 1.0], (nz, ny, 1))
+    gx = gx + np.where(slab, fs, 0.0)
+    bx = (up(Az, 1) - Az) / h - (up(Ay, 0) - Ay) / h + gx
+    by = (up(Ax, 0) - Ax) / h - (up(Az, 2) - Az) / h + gy
+    bz = (up(Ay, 2) - Ay) / h - (up(Ax, 1) - Ax) / h + gz
+    u = np.zeros((11,) + shape)
+    u[5], u[6], u[7] = bx, by, bz
+    u[8], u[9], u[10] = up(bx, 2), up(by, 1), up(bz, 0)
+    B2 = 0.25 * ((u[5] + u[8]) ** 2 + (u[6] + u[9]) ** 2 + (u[7] + u[10]) ** 2)
+    # density, velocity, specific internal energy as in floor_state (3-D)
+    rho = 10.0 ** rng.uniform(np.log10(0.1 * smallr), 0.0, shape)
+    eint = 10.0 ** rng.uniform(-5.0, 0.0, shape)
+    dirs = rng.standard_normal((3,) + shape)
+    vel = dirs * (10.0 ** rng.uniform(-1.0, 0.5, shape) / np.sqrt((dirs ** 2).sum(axis=0)))
+    vac = rng.random(shape) < 0.03
+    for d in range(3):
+        ax = 2 - d
+        for s in (-1, 1):
+            nb = np.roll(vac, s, axis=ax) & ~vac
+            k = int(nb.sum())
+            rho[nb] = rng.uniform(0.5, 2.0, k)
+            for e in range(3):
+                vel[e][nb] = s * rng.uniform(1.0, 3.0, k) if e == d else rng.uniform(-1.0, 1.0, k)
+    rho[vac] = rng.uniform(0.1, 0.9, int(vac.sum())) * smallr
+    vel[1][slab] *= slab_vt
+    vel[2][slab] *= slab_vt
+    P = (gamma - 1) * rho * eint
+    # the slab: vA^2 / c_s^2 = B^2 / (gamma P) away from 1 on both sides
+    ratio = np.where(rng.random(shape) < 0.5, rng.uniform(2.0, 20.0, shape), rng.uniform(0.05, 0.5, shape))
+    P[slab] = (B2 / (gamma * ratio))[slab]
+    kinds = rng.random(shape)
+    hyp = (kinds < 0.06) & ~vac & ~slab
+    cold = (kinds >= 0.06) & (kinds < 0.12) & ~vac & ~quiet & (B2 > 1e-4)
+    mdom = (kinds >= 0.12) & (kinds < 0.17) & ~vac & ~quiet & (B2 > 1e-2)
+    k = int(hyp.sum())
+    rho[hyp] = 10.0 ** rng.uniform(np.log10(smallr), 0.0, k)
+    hdir = rng.standard_normal((3, k))
+    hdir /= np.sqrt((hdir ** 2).sum(axis=0))
+    c0 = np.sqrt(gamma * (gamma - 1) * 10.0 ** rng.uniform(-4.0, -2.0, k))
+    for e in range(3):
+        vel[e][hyp] = hdir[e] * c0 * rng.uniform(10.0, 100.0, k)
+    rho[mdom] = rng.uniform(0.1, 10.0, int(mdom.sum())) * smallr
+    P[mdom] = (0.5 * B2 * 10.0 ** rng.uniform(-20.0, -6.0, shape))[mdom]
+    u[0] = rho
+    for c in range(3):
+        u[1 + c] = rho * vel[c]
+    ekin = 0.5 * rho * (vel[0] ** 2 + vel[1] ** 2 + vel[2] ** 2)
+    emag = 0.5 * B2
+    u[4] = P / (gamma - 1.0) + ekin + emag
+    delta = rng.choice([0.0, 1e-14, 1e-3], shape)
+    u[4][hyp] = (ekin * (1.0 - delta) + emag)[hyp]
+    u[4][cold] = (ekin + emag * (1.0 - delta))[cold]
+    return u
+
+
+def mhd_floor_counts(u, smallr, smallc, gamma=5.0 / 3.0):
+    """(cells with rho < smallr, cells whose raw pressure (gamma-1) (E - ekin - emag) with rho floored is below smallp =
+    smallr smallc^2 / gamma, field-free cells (all six faces 0), field-aligned cells (B = (bx, 0, 0), bx != 0) with vA > c_s)
+    of a dense MHD state [11][nz][ny][nx]: the cells on which the ctoprim floors of the MHD kernels fire and where the field
+    degenerates"""
+    r = np.maximum(u[0], smallr)
+    ekin = 0.5 * (u[1] ** 2 + u[2] ** 2 + u[3] ** 2) / r
+    B2 = 0.25 * ((u[5] + u[8]) ** 2 + (u[6] + u[9]) ** 2 + (u[7] + u[10]) ** 2)
+    smallp = smallr * smallc ** 2 / gamma
+    praw = (gamma - 1) * (u[4] - ekin - 0.5 * B2)
+    free = (u[5:11] == 0).all(axis=0)
+    aligned = (u[6] == 0) & (u[9] == 0) & (u[7] == 0) & (u[10] == 0) & (u[5] != 0)
+    fast = aligned & (B2 / r > gamma * np.maximum(praw, smallp) / r)
+    return int((u[0] < smallr).sum()), int((praw < smallp).sum()), int(free.sum()), int(fast.sum())
+
+
+def fill_mhd_floor_cells(run, floors, seed, field_scale=1.0):
+    """put floor-state draws on every cell of an MHD AMR run (run.uold, 11 x ncell): rho, the momentum and E are overwritten, the
+    face fields are the run's own (scaled by field_scale; 0 gives a field-free tree), so div B = 0 and the coarse/fine face
+    consistency are kept; E is recomputed from those faces.  Sets the run's floors to helpers.FLOORS[floors] (both the hydro and
+    the MHD parameter blocks) and asserts that the density and pressure floors fire.  Returns (smallr, smallc)."""
+    smallr, smallc = FLOORS[floors]
+    gamma = run.pm.gamma
+    run.p.smallr, run.p.smallc = smallr, smallc
+    run.pm.smallr, run.pm.smallc = smallr, smallc
+    U = run.uold.reshape(11, run.ncell)
+    n = run.ncell
+    rng = np.random.default_rng(seed)
+    U[5:11] *= field_scale
+    B2 = 0.25 * ((U[5] + U[8]) ** 2 + (U[6] + U[9]) ** 2 + (U[7] + U[10]) ** 2)
+    rho = 10.0 ** rng.uniform(np.log10(0.1 * smallr), 0.0, n)
+    dirs = rng.standard_normal((3, n))
+    vel = dirs * (10.0 ** rng.uniform(-1.0, 0.5, n) / np.sqrt((dirs ** 2).sum(axis=0)))
+    P = (gamma - 1) * rho * 10.0 ** rng.uniform(-5.0, 0.0, n)
+    kinds = rng.random(n)
+    hyp = kinds < 0.08
+    c0 = np.sqrt(gamma * (gamma - 1) * 10.0 ** rng.uniform(-4.0, -2.0, n))
+    vel[:, hyp] *= (c0 * rng.uniform(10.0, 100.0, n) / np.sqrt((vel ** 2).sum(axis=0)))[hyp]
+    mdom = (kinds >= 0.08) & (kinds < 0.14) & (B2 > 1e-2)
+    rho[mdom] = rng.uniform(0.1, 10.0, int(mdom.sum())) * smallr
+    P[mdom] = (0.5 * B2 * 10.0 ** rng.uniform(-20.0, -6.0, n))[mdom]
+    ekin = 0.5 * rho * (vel ** 2).sum(axis=0)
+    delta = rng.choice([0.0, 1e-14, 1e-3], n)
+    U[0] = rho
+    U[1:4] = rho * vel
+    U[4] = P / (gamma - 1) + ekin + 0.5 * B2
+    U[4][hyp] = (ekin * (1 - delta) + 0.5 * B2)[hyp]
+    cold = (kinds >= 0.14) & (kinds < 0.22)
+    U[4][cold] = (ekin + 0.5 * B2 * (1 - delta))[cold]
+    r = np.maximum(rho, smallr)
+    praw = (gamma - 1) * (U[4] - 0.5 * (U[1] ** 2 + U[2] ** 2 + U[3] ** 2) / r - 0.5 * B2)
+    nrho, np_ = int((rho < smallr).sum()), int((praw < smallr * smallc ** 2 / gamma).sum())
+    assert min(nrho, np_) >= 0.02 * n, (nrho, np_)
+    return smallr, smallc
+
+
 def level_slots(mesh, l, u, nvar):
     """The octs of level l of an oracle mesh (active and boundary octs) in the dense-box slot layout of the device (plan_level:
     lattice order of the oct positions over the box spanned by them): returns uin [nvar][2^ndim][nslot] and the (igrid, slot)
@@ -351,11 +502,12 @@ class MhdCase:
     """MHD run set-up: oracle mesh + MHD params + the Fortran-side arrays (AmrCommons of an MHD build)."""
 
     def __init__(self, level, riemann="hlld", riemann2d="llf", slope_type=1, slope_mag_type=-1, bound=(0,) * 6, order=0, seed=1,
-                 boxlen=1.0, gamma=5.0 / 3.0, courant_factor=0.8, slope_theta=1.5, coarse=(1, 1, 1)):
+                 boxlen=1.0, gamma=5.0 / 3.0, courant_factor=0.8, slope_theta=1.5, coarse=(1, 1, 1), smallr=1e-10, smallc=1e-10):
         self.ndim, self.level, self.nvar, self.nvs = 3, level, 8, 11
         self.mesh = orc.Mesh(3, level, bound, order, seed, coarse=coarse)
         self.p = orc.make_mhd_params(slope_type=slope_type, slope_mag_type=slope_mag_type, riemann=riemann, riemann2d=riemann2d,
-                                     gamma=gamma, courant_factor=courant_factor, boxlen=boxlen, slope_theta=slope_theta)
+                                     gamma=gamma, courant_factor=courant_factor, boxlen=boxlen, slope_theta=slope_theta,
+                                     smallr=smallr, smallc=smallc)
         self.riemann, self.riemann2d, self.slope_type, self.slope_mag_type = riemann, riemann2d, slope_type, slope_mag_type
         self.u = self.mesh.new_state(11)
 

@@ -609,6 +609,42 @@ void devnum_mhd_sweep_box(const int* n, const int* shell, int r1d, int r2d, int 
   emulate_serial(mhd_update_kernel, a, 8, 256);
 }
 
+// the stand-alone MHD Courant scan (mhd_courant_kernel, mhd_dense.cuh) on a box laid out like devnum_mhd_sweep_box, launched with
+// nblocks CTAs of 256 threads like launch_mhd_courant: part[5][nblocks] = per-block min dt, sum rho, sum E, sum eint, sum emag
+struct MhdCourantHost { const double* u; DenseGeom g; MPhys P; double dx; double* part; };
+void devnum_mhd_courant(const int* n, const int* shell, int nblocks, const double* u, double dx, double gamma, double smallr,
+                        double smallc, double cfl, double* part) {
+  MhdCourantHost a;
+  a.u = u; a.g = box_geom(3, n, shell); a.P = make_mphys(gamma, smallr, smallc); a.P.courant_factor = cfl; a.dx = dx; a.part = part;
+  emulate_launch([](const MhdCourantHost& c) { mhd_courant_kernel(c.u, c.g, c.P, c.dx, c.part); }, a, nblocks, 256);
+}
+
+// make_boundary_hydro of the dense MHD path (mhd_boundary_kernel) for one boundary region of such a box: the MhdBoundArgs that
+// launch_boundaries (rgpu_api.cu) builds for boundary type bt and the region's oct slots; u [11][8][nslot] is updated in place
+void devnum_mhd_boundary(const int* n, const int* shell, int bt, const int* slots, int nreg, double* u, double smallr) {
+  static const int ref_x[8] = {2, 1, 4, 3, 6, 5, 8, 7}, ref_y[8] = {3, 4, 1, 2, 7, 8, 5, 6}, ref_z[8] = {5, 6, 7, 8, 1, 2, 3, 4};
+  static const int fre[6][8] = {{1, 1, 3, 3, 5, 5, 7, 7}, {2, 2, 4, 4, 6, 6, 8, 8}, {1, 2, 1, 2, 5, 6, 5, 6},
+                                {3, 4, 3, 4, 7, 8, 7, 8}, {1, 2, 3, 4, 1, 2, 3, 4}, {5, 6, 7, 8, 5, 6, 7, 8}};
+  static const int alt_[6][8] = {{-2, -1, -2, -1, -2, -1, -2, -1}, {1, 2, 1, 2, 1, 2, 1, 2}, {-2, -2, -1, -1, -2, -2, -1, -1},
+                                 {1, 1, 2, 2, 1, 1, 2, 2}, {-2, -2, -2, -2, -1, -1, -1, -1}, {1, 1, 1, 1, 2, 2, 2, 2}};
+  const DenseGeom g = box_geom(3, n, shell);
+  const long long str[3] = {1, g.nox, (long long)g.nox * g.noy};
+  const int dir = bt - 10 * (bt / 10), d = (dir - 1) / 2;
+  MhdBoundArgs m;
+  std::memset(&m, 0, sizeof m);
+  m.n = nreg; m.slots = slots; m.nslot = g.nslot;
+  m.nbr_off = (dir % 2 == 1) ? str[d] : -str[d];
+  const int* ir = (bt / 10 == 0) ? (d == 0 ? ref_x : d == 1 ? ref_y : ref_z) : fre[dir - 1];
+  for (int i = 0; i < 8; i++) { m.ind_ref[i] = ir[i]; m.ind_normal[i] = fre[dir - 1][i]; m.alt[i] = alt_[dir - 1][i]; }
+  m.gs[0] = m.gs[1] = m.gs[2] = 1.0;
+  if (bt >= 1 && bt <= 6) m.gs[d] = -1.0;
+  m.kind = bt / 10; m.gdim = d + 1;
+  m.iperp1 = (dir % 2 == 1) ? 4 + m.gdim : 7 + m.gdim;
+  m.smallr = smallr;
+  struct B { double* u; MhdBoundArgs m; } b{u, m};
+  emulate_serial([](const B& x) { mhd_boundary_kernel(x.u, x.m); }, b, (nreg * 8 + 127) / 128, 128);
+}
+
 void devnum_mhd_sweep(int N, int r1d, int r2d, int sl, const double* uin, double* uout, double dt, double dx, double gamma,
                       double smallr, double smallc, int slope_type, int slope_mag_type) {
   const int n[3] = {N, N, N};

@@ -221,38 +221,188 @@ def _mhd_states(rng, n):
     return np.ascontiguousarray(ql), np.ascontiguousarray(qr)
 
 
+MHD_CLASSES = ("vacuum", "pfloor", "free", "aligned_fast", "aligned_slow", "mdom", "tiny_bt")
+
+
+def _mhd_degenerate_states(rng, k, gamma=5 / 3.):
+    """k left/right pairs per degenerate class, in the solver order of _mhd_states (equal B_n on both sides):
+    vacuum -- densities 1e-12-1e-3, one side or both, below smallr under both helpers.FLOORS settings;
+    pfloor -- pressure 0 or 1e-40 on one side or both (hydro_acoustic's pressure floor);
+    free -- B = 0 on both sides; half of them strong rarefactions out of thin, cold gas (rstar / cstar of hydro_acoustic floored);
+    aligned_fast / aligned_slow -- B = (B_n, 0, 0) with vA^2 / c_s^2 in 2-20 / 0.05-0.5 (never 1), a third of the pairs with
+      equal sides (the HLLD star state degenerates: |estar| < 1e-4 B_n^2), a third nearly equal;
+    mdom -- near-vacuum magnetically dominated, plasma beta 1e-20-1e-6;
+    tiny_bt -- tangential fields 1e-16-1e-6 next to an O(1) normal field.
+    Returns ql, qr and {class: row slice}."""
+    rows, cls = [], {}
+    for name in MHD_CLASSES:
+        l, r = _mhd_states(rng, k)
+        if name == "vacuum":
+            l[:, 0] = 10.0 ** rng.uniform(-12, -3, k)
+            both = rng.random(k) < 0.5
+            r[both, 0] = 10.0 ** rng.uniform(-12, -3, int(both.sum()))
+        elif name == "pfloor":
+            l[:, 1] = rng.choice([0.0, 1e-40], k)
+            both = rng.random(k) < 0.5
+            r[both, 1] = rng.choice([0.0, 1e-40], int(both.sum()))
+        elif name == "free":
+            l[:, [3, 5, 7]] = 0.0
+            r[:, [3, 5, 7]] = 0.0
+            h = k // 2
+            l[:h, 0], r[:h, 0] = 10.0 ** rng.uniform(-12, -3, h), 10.0 ** rng.uniform(-12, -3, h)
+            l[:h, 1], r[:h, 1] = 10.0 ** rng.uniform(-30, -12, h), 10.0 ** rng.uniform(-30, -12, h)
+            l[:h, 2], r[:h, 2] = -(10.0 ** rng.uniform(-1, 2, h)), 10.0 ** rng.uniform(-1, 2, h)
+        elif name in ("aligned_fast", "aligned_slow"):
+            for q in (l, r):
+                q[:, [5, 7]] = 0.0
+            bn = rng.uniform(0.2, 2.0, k) * rng.choice([-1.0, 1.0], k)
+            l[:, 3] = r[:, 3] = bn
+            ratio = rng.uniform(2.0, 20.0, k) if name == "aligned_fast" else rng.uniform(0.05, 0.5, k)
+            for q in (l, r):
+                q[:, 1] = bn ** 2 / (gamma * ratio)
+            t = k // 3
+            r[:t] = l[:t]
+            r[t:2 * t] = l[t:2 * t] * (1 + 1e-6 * rng.standard_normal((t, 8)))
+            r[t:2 * t, [3, 5, 7]] = l[t:2 * t, [3, 5, 7]]
+            for q in (l, r):
+                q[:, 1] = q[:, 3] ** 2 / (gamma * ratio)
+            zt = rng.random(k) < 0.5                          # half of them move along the field only
+            l[zt, 4] = l[zt, 6] = r[zt, 4] = r[zt, 6] = 0.0
+        elif name == "mdom":
+            for q in (l, r):
+                q[:, 0] = 10.0 ** rng.uniform(-11, -6, k)
+                q[:, 1] = 0.5 * (q[:, 3] ** 2 + q[:, 5] ** 2 + q[:, 7] ** 2) * 10.0 ** rng.uniform(-20, -6, k)
+        else:
+            for q in (l, r):
+                q[:, [5, 7]] = rng.standard_normal((k, 2)) * 10.0 ** rng.uniform(-16, -6, (k, 1))
+            bn = rng.uniform(0.2, 2.0, k)
+            l[:, 3] = r[:, 3] = bn
+        cls[name] = slice(len(rows) * k, (len(rows) + 1) * k)
+        rows.append((l, r))
+    ql = np.concatenate([a for a, _ in rows])
+    qr = np.concatenate([b for _, b in rows])
+    return np.ascontiguousarray(ql), np.ascontiguousarray(qr), cls
+
+
+def _assert_mhd_classes_present(ql, qr, cls, smallr, smallc, gamma=5 / 3.):
+    """every degenerate class of _mhd_degenerate_states is in the inputs, and its defining property holds"""
+    smallp = smallr * smallc ** 2 / gamma
+    q = {n: (ql[s], qr[s]) for n, s in cls.items()}
+    assert (q["vacuum"][0][:, 0] < smallr).sum() >= 10
+    assert (q["pfloor"][0][:, 1] < smallp).all()
+    assert all((a[:, [3, 5, 7]] == 0).all() for a in q["free"])
+    for name, fast in (("aligned_fast", True), ("aligned_slow", False)):
+        l, r = q[name]
+        assert (l[:, [5, 7]] == 0).all() and (r[:, [5, 7]] == 0).all() and (l[:, 3] != 0).all()
+        va2, cs2 = l[:, 3] ** 2 / l[:, 0], gamma * l[:, 1] / l[:, 0]
+        assert ((va2 > 1.5 * cs2) if fast else (va2 < 0.6 * cs2)).all()
+        assert (l == r).all(axis=1).sum() > 0
+    l, _ = q["mdom"]
+    assert (2 * l[:, 1] / (l[:, 3] ** 2 + l[:, 5] ** 2 + l[:, 7] ** 2)).min() < 1e-18
+    assert (np.abs(q["tiny_bt"][0][:, 5]) < 1e-12).sum() > 0
+
+
 @pytest.mark.parametrize("solver", ["llf", "roe", "hll", "hlld", "upwind", "hydro"])
 def test_mhd_riemann_device_formulas_equal_oracle(orc, dev, solver):
     """lax_friedrich / athena_roe (restructured on the device: left eigenvectors column by column, shared reciprocals) / hll /
-    hlld / upwind / hydro_acoustic of mhd_device.cuh == the oracle's restatement of mhd/godunov_utils.f90, bit for bit"""
-    n = 20000
-    ql, qr = _mhd_states(np.random.default_rng(40 + len(solver)), n)
-    fg = np.zeros((n, 9))
-    dev.devnum_mhd_riemann(orc.MHD_RIEMANN[solver], n, orc.dptr(ql), orc.dptr(qr), orc.dptr(fg), 5 / 3., 1e-10, 1e-10)
-    pm = orc.make_mhd_params(riemann=solver, gamma=5 / 3.)
+    hlld / upwind / hydro_acoustic of mhd_device.cuh == the oracle's restatement of mhd/godunov_utils.f90, bit for bit on every
+    row and no row NaN, under both helpers.FLOORS settings: random pairs plus the degenerate
+    classes of _mhd_degenerate_states (near-vacuum, floored pressure, zero field, field along the normal with vA above and below
+    c_s, beta down to 1e-20, tiny tangential fields).  Roe falls back to the LLF flux on some rows (unphysical intermediate
+    state); the count of those rows is asserted and reported."""
+    n, k = 20000, 600
+    rng = np.random.default_rng(40 + len(solver))
+    ql0, qr0 = _mhd_states(rng, n)
+    qld, qrd, cls = _mhd_degenerate_states(rng, k)
+    ql, qr = np.concatenate([ql0, qld]), np.concatenate([qr0, qrd])
+    cls = {c: slice(s.start + n, s.stop + n) for c, s in cls.items()}
+    n = len(ql)
     L = orc.lib()
     L.orc_mhd_riemann.argtypes = [C.POINTER(orc.MhdParams)] + [C.POINTER(C.c_double)] * 3
-    ref = np.zeros((n, 9))
-    for i in range(n):
-        L.orc_mhd_riemann(C.byref(pm), orc.dptr(ql[i]), orc.dptr(qr[i]), orc.dptr(ref[i]))
-    nused = 8 if solver != "hlld" else 8
-    good = np.isfinite(ref[:, :nused]).all(axis=1)
-    assert good.mean() > 0.99
-    assert np.array_equal(fg[good, :nused], ref[good, :nused])
+    for smallr, smallc in FLOORS.values():
+        _assert_mhd_classes_present(ql, qr, cls, smallr, smallc)
+        fg = np.zeros((n, 9))
+        dev.devnum_mhd_riemann(orc.MHD_RIEMANN[solver], n, orc.dptr(ql), orc.dptr(qr), orc.dptr(fg), 5 / 3., smallr, smallc)
+        pm = orc.make_mhd_params(riemann=solver, gamma=5 / 3., smallr=smallr, smallc=smallc)
+        ref = np.zeros((n, 9))
+        for i in range(n):
+            L.orc_mhd_riemann(C.byref(pm), orc.dptr(ql[i]), orc.dptr(qr[i]), orc.dptr(ref[i]))
+        nan = ~np.isfinite(ref[:, :8]).all(axis=1)
+        print(f"{solver} smallr={smallr:g}: {int(nan.sum())} non-finite rows of {n}")
+        assert not nan.any()
+        assert np.array_equal(fg[:, :8], ref[:, :8], equal_nan=True), \
+            [c for c, s in cls.items() if not np.array_equal(fg[s, :8], ref[s, :8], equal_nan=True)]
+        if solver == "roe":
+            fl = np.zeros((n, 9))
+            dev.devnum_mhd_riemann(orc.MHD_RIEMANN["llf"], n, orc.dptr(ql), orc.dptr(qr), orc.dptr(fl), 5 / 3., smallr, smallc)
+            nllf = int((fl[:, :8] == fg[:, :8]).all(axis=1).sum())
+            print(f"roe rows equal to the LLF flux (unphysical intermediate state): {nllf}")
+            assert nllf > 0
 
 
-@pytest.mark.parametrize("solver2d", ["llf", "roe", "upwind", "hll", "hlla", "hlld"])
-def test_mhd_corner_emf_device_formulas_equal_oracle(orc, dev, solver2d):
-    """emf_edge<R2D> (cmp_mag_flx, mhd/umuscl.f90:1453) for the E_z call: the four corner states in the reference's dummy-argument
-    order; the oracle is called with the cell-order corner states of the same edge"""
-    n = 10000
-    rng = np.random.default_rng(77 + len(solver2d))
-    RT, RB, LT, LB = (np.zeros((n, 8)) for _ in range(4))            # (rho, u, v, w, P, A, B, C)
+def _emf_corners(rng, n):
+    """RT, RB, LT, LB corner states (rho, u, v, w, P, A, B, C) of the E_z edge"""
+    RT, RB, LT, LB = (np.zeros((n, 8)) for _ in range(4))
     for q in (RT, RB, LT, LB):
         q[:, 0] = 10.0 ** rng.uniform(-1, 1, n)
         q[:, 4] = 10.0 ** rng.uniform(-2, 1, n)
         q[:, 1:4] = rng.standard_normal((n, 3))
         q[:, 5:8] = rng.standard_normal((n, 3))
+    return RT, RB, LT, LB
+
+
+def _emf_degenerate_corners(rng, k, gamma=5 / 3.):
+    """k edges per class: vacuum (corner densities 1e-12-1e-3), free (all fields zero), tiny (fields 1e-16-1e-6: the Alfven
+    speeds of 2-D HLLD fall below smallc), aligned (B along x or y only, vA^2 / c_s^2 in 2-20 or 0.05-0.5), mdom (beta down to
+    1e-20); returns the four corner arrays and {class: row slice}"""
+    parts, cls = [], {}
+    for j, name in enumerate(("vacuum", "free", "tiny", "aligned", "mdom")):
+        c = _emf_corners(rng, k)
+        for q in c:
+            if name == "vacuum":
+                q[:, 0] = 10.0 ** rng.uniform(-12, -3, k)
+            elif name == "free":
+                q[:, 5:8] = 0.0
+            elif name == "tiny":
+                q[:, 5:8] *= 10.0 ** rng.uniform(-16, -6, (k, 1))
+            elif name == "mdom":
+                q[:, 0] = 10.0 ** rng.uniform(-11, -6, k)
+                q[:, 4] = 0.5 * (q[:, 5:8] ** 2).sum(axis=1) * 10.0 ** rng.uniform(-20, -6, k)
+        if name == "aligned":
+            ax = np.where(rng.random(k) < 0.5, 5, 6)
+            b = rng.uniform(0.2, 2.0, k)
+            ratio = np.where(rng.random(k) < 0.5, rng.uniform(2.0, 20.0, k), rng.uniform(0.05, 0.5, k))
+            for q in c:
+                q[:, 5:8] = 0.0
+                q[np.arange(k), ax] = b
+                q[:, 4] = b ** 2 / (gamma * ratio)
+        cls[name] = slice(j * k, (j + 1) * k)
+        parts.append(c)
+    return tuple(np.concatenate([p[i] for p in parts]) for i in range(4)), cls
+
+
+@pytest.mark.parametrize("solver2d", ["llf", "roe", "upwind", "hll", "hlla", "hlld"])
+def test_mhd_corner_emf_device_formulas_equal_oracle(orc, dev, solver2d):
+    """emf_edge<R2D> (cmp_mag_flx, mhd/umuscl.f90:1453) for the E_z call: the four corner states in the reference's dummy-argument
+    order; the oracle is called with the cell-order corner states of the same edge.  Random edges plus near-vacuum, field-free,
+    tiny-field (the smallc floor of the 2-D HLLD Alfven speeds), axis-aligned and magnetically dominated edges, under both
+    helpers.FLOORS settings: every row bit for bit and finite on both sides"""
+    n, k = 10000, 400
+    rng = np.random.default_rng(77 + len(solver2d))
+    RT, RB, LT, LB = _emf_corners(rng, n)
+    (dRT, dRB, dLT, dLB), cls = _emf_degenerate_corners(rng, k)
+    RT, RB, LT, LB = (np.concatenate([a, b]) for a, b in ((RT, dRT), (RB, dRB), (LT, dLT), (LB, dLB)))
+    cls = {c: slice(s.start + n, s.stop + n) for c, s in cls.items()}
+    n = len(RT)
+    for q in (RT, RB, LT, LB):
+        assert (q[cls["free"], 5:8] == 0).all() and (np.abs(q[cls["tiny"], 5:8]) < 1e-5).all()
+        assert (q[cls["vacuum"], 0] < 1e-10).sum() > 0
+        a = q[cls["aligned"]]
+        assert ((a[:, 5:8] != 0).sum(axis=1) == 1).all() and (a[:, 7] == 0).all()
+        va2, cs2 = (a[:, 5:8] ** 2).sum(axis=1) / a[:, 0], 5 / 3. * a[:, 4] / a[:, 0]
+        assert ((va2 > 1.5 * cs2) | (va2 < 0.6 * cs2)).all() and (va2 > 1.5 * cs2).any() and (va2 < 0.6 * cs2).any()
+        md = q[cls["mdom"]]
+        assert (2 * md[:, 4] / (md[:, 5:8] ** 2).sum(axis=1)).min() < 1e-18
     # face fields are shared: A (x-face) by the left/right pair, B (y-face) by the top/bottom pair (umuscl.f90:1506-1541)
     lp1, lp2, lor, bp1, bp2, bor = 2, 3, 4, 6, 7, 8
     LL, RL, LR, RR = (np.zeros((n, 8)) for _ in range(4))
@@ -263,39 +413,85 @@ def test_mhd_corner_emf_device_formulas_equal_oracle(orc, dev, solver2d):
     LR[:, 5] = RR[:, 5] = 0.5 * (RB[:, bp1 - 1] + LB[:, bp1 - 1])
     LL[:, 6] = LR[:, 6] = 0.5 * (RT[:, bp2 - 1] + RB[:, bp2 - 1])
     RL[:, 6] = RR[:, 6] = 0.5 * (LT[:, bp2 - 1] + LB[:, bp2 - 1])
-    emf = np.zeros(n)
-    dev.devnum_mhd_emf(orc.MHD_RIEMANN2D[solver2d], n, *(orc.dptr(np.ascontiguousarray(a)) for a in (LL, RL, LR, RR)), orc.dptr(emf),
-                       5 / 3., 1e-10, 1e-10)
-    pm = orc.make_mhd_params(riemann2d=solver2d, gamma=5 / 3.)
     L = orc.lib()
     L.orc_mhd_emf.restype = C.c_double
     L.orc_mhd_emf.argtypes = [C.POINTER(orc.MhdParams)] + [C.POINTER(C.c_double)] * 4 + [C.c_int]
-    ref = np.array([L.orc_mhd_emf(C.byref(pm), orc.dptr(RT[i]), orc.dptr(RB[i]), orc.dptr(LT[i]), orc.dptr(LB[i]), 2) for i in range(n)])
-    good = np.isfinite(ref)
-    assert good.mean() > 0.99
-    assert np.array_equal(emf[good], ref[good])
+    for smallr, smallc in FLOORS.values():
+        emf = np.zeros(n)
+        dev.devnum_mhd_emf(orc.MHD_RIEMANN2D[solver2d], n, *(orc.dptr(np.ascontiguousarray(a)) for a in (LL, RL, LR, RR)),
+                           orc.dptr(emf), 5 / 3., smallr, smallc)
+        pm = orc.make_mhd_params(riemann2d=solver2d, gamma=5 / 3., smallr=smallr, smallc=smallc)
+        ref = np.array([L.orc_mhd_emf(C.byref(pm), orc.dptr(RT[i]), orc.dptr(RB[i]), orc.dptr(LT[i]), orc.dptr(LB[i]), 2)
+                        for i in range(n)])
+        nan = ~np.isfinite(ref)
+        print(f"{solver2d} smallr={smallr:g}: {int(nan.sum())} non-finite rows of {n}")
+        assert not nan.any()
+        assert np.array_equal(emf, ref, equal_nan=True), \
+            [c for c, s in cls.items() if not np.array_equal(emf[s], ref[s], equal_nan=True)]
+
+
+def _mhd_cmpdt_cells(rng, n, k=300, gamma=5 / 3.):
+    """n ordinary cells [11] plus k cells per class: densities 1e-13-1e-4 (below smallr), cold magnetised E = ekin + emag (1 -
+    delta), field-free, field along x, y or z with vA^2 / c_s^2 in 2-20 or 0.05-0.5, magnetically dominated near-vacuum"""
+    u = np.zeros((n + 5 * k, 11))
+    u[:, 0] = 10.0 ** rng.uniform(-2, 1, len(u))
+    vel = rng.standard_normal((len(u), 3)) * 2
+    u[:, 5:8] = rng.standard_normal((len(u), 3))
+    u[:, 8:11] = u[:, 5:8] + 0.1 * rng.standard_normal((len(u), 3))
+    P = 10.0 ** rng.uniform(-3, 1, len(u))
+    s = [slice(n + j * k, n + (j + 1) * k) for j in range(5)]
+    u[s[0], 0] = 10.0 ** rng.uniform(-13, -4, k)
+    u[s[2], 5:11] = 0.0
+    ax = rng.integers(0, 3, k)
+    b = rng.uniform(0.2, 2.0, k)
+    u[s[3], 5:11] = 0.0
+    rows = np.arange(s[3].start, s[3].stop)
+    u[rows, 5 + ax] = u[rows, 8 + ax] = b
+    ratio = np.where(rng.random(k) < 0.5, rng.uniform(2.0, 20.0, k), rng.uniform(0.05, 0.5, k))
+    P[s[3]] = b ** 2 / (gamma * ratio)
+    u[s[4], 0] = 10.0 ** rng.uniform(-11, -6, k)
+    bc = 0.5 * (u[:, 5:8] + u[:, 8:11])
+    emag = 0.5 * (bc ** 2).sum(axis=1)
+    P[s[4]] = (emag * 10.0 ** rng.uniform(-20, -6, len(u)))[s[4]]
+    u[:, 1:4] = u[:, :1] * vel
+    ekin = 0.5 * u[:, 0] * (vel ** 2).sum(axis=1)
+    u[:, 4] = P / (gamma - 1) + ekin + emag
+    u[s[1], 4] = (ekin + emag * (1 - rng.choice([0.0, 1e-14, 1e-3], len(u))))[s[1]]
+    return np.ascontiguousarray(u), s
 
 
 def test_mhd_cmpdt_device_formula_equals_oracle(orc, dev):
-    n = 5000
+    """cmpdt of the MHD build (mhd/godunov_utils.f90:5-111) on ordinary cells plus cells below smallr, cold magnetised cells whose
+    pressure floor fires, field-free, axis-aligned and magnetically dominated cells, under both helpers.FLOORS settings: every
+    time step bit for bit, the oracle finite"""
     rng = np.random.default_rng(9)
-    u = np.zeros((n, 11))
-    u[:, 0] = 10.0 ** rng.uniform(-2, 1, n)
-    vel = rng.standard_normal((n, 3)) * 2
-    u[:, 1:4] = u[:, :1] * vel
-    u[:, 5:8] = rng.standard_normal((n, 3))
-    u[:, 8:11] = u[:, 5:8] + 0.1 * rng.standard_normal((n, 3))
-    bc = 0.5 * (u[:, 5:8] + u[:, 8:11])
-    u[:, 4] = 10.0 ** rng.uniform(-3, 1, n) / (5 / 3. - 1) + 0.5 * u[:, 0] * (vel ** 2).sum(axis=1) + 0.5 * (bc ** 2).sum(axis=1)
-    dt = np.zeros(n)
+    u, s = _mhd_cmpdt_cells(rng, 5000)
+    n = len(u)
     dx = 1.0 / 64
-    dev.devnum_mhd_cmpdt(n, orc.dptr(np.ascontiguousarray(u)), dx, orc.dptr(dt), 5 / 3., 1e-10, 1e-10, 0.8)
-    pm = orc.make_mhd_params(gamma=5 / 3., courant_factor=0.8)
     L = orc.lib()
     L.orc_mhd_cmpdt_cell.restype = C.c_double
     L.orc_mhd_cmpdt_cell.argtypes = [C.POINTER(orc.MhdParams), C.POINTER(C.c_double), C.c_double]
-    ref = np.array([L.orc_mhd_cmpdt_cell(C.byref(pm), orc.dptr(u[i].copy()), dx) for i in range(n)])
-    assert np.array_equal(dt, ref)
+    for smallr, smallc in FLOORS.values():
+        dt = np.zeros(n)
+        dev.devnum_mhd_cmpdt(n, orc.dptr(u), dx, orc.dptr(dt), 5 / 3., smallr, smallc, 0.8)
+        pm = orc.make_mhd_params(gamma=5 / 3., courant_factor=0.8, smallr=smallr, smallc=smallc)
+        ref = np.array([L.orc_mhd_cmpdt_cell(C.byref(pm), orc.dptr(u[i].copy()), dx) for i in range(n)])
+        assert np.isfinite(ref).all()
+        assert np.array_equal(dt, ref)
+        nrho, npr, nfree, nfast = _cmpdt_cell_counts(u, smallr, smallc)
+        assert min(nrho, npr, nfree, nfast) >= 50, (nrho, npr, nfree, nfast)
+
+
+def _cmpdt_cell_counts(u, smallr, smallc, gamma=5 / 3.):
+    """mhd_floor_counts of the cells u [n][11], with the field-aligned count taken over the three axes"""
+    from helpers import mhd_floor_counts
+    nrho, npr, nfree, _ = mhd_floor_counts(u.T.reshape(11, 1, 1, -1), smallr, smallc)
+    nfast = 0
+    for ax in range(3):
+        p3 = np.array([ax, (ax + 1) % 3, (ax + 2) % 3])        # the field axis becomes x
+        w = u[:, np.concatenate([[0], 1 + p3, [4], 5 + p3, 8 + p3])]
+        nfast += mhd_floor_counts(w.T.reshape(11, 1, 1, -1), smallr, smallc)[3]
+    return nrho, npr, nfree, nfast
 
 
 @pytest.mark.parametrize("solver", ["hllc", "llf", "exact", "acoustic", "hll"])
@@ -1462,3 +1658,207 @@ def test_dense_sweep_amr_variant_emulated_at_the_floors(orc, dev, floors, solver
     """sweep_dense_kernel<..., AMRV=true> on a 48x32x16 base level holding a floor_state, a tenth of its cells marked refined:
     equals set_unew + godunov_fine of the oracle, bit for bit"""
     _dense_amr_box_compare(orc, dev, (3, 2, 1), (0,) * 6, solver, 5, floors=floors)
+
+
+# ---- MHD at the floors and where the field degenerates (helpers.mhd_floor_state, helpers.fill_mhd_floor_cells) ----
+MHD_FLOOR_PAIRS = [("roe", "llf", 0, 0), ("hlld", "hlld", 1, 1), ("llf", "llf", 2, 2), ("hll", "hll", 1, 1), ("hlld", "roe", 2, 2),
+                   ("upwind", "upwind", 1, 1), ("hydro", "hlla", 1, 1), ("hlld", "hlld", 3, 1), ("roe", "llf", 7, 2),
+                   ("hll", "hlld", 8, 1)]
+
+
+def _mhd_floor_case(coarse, level, bound, r1d, r2d, st, smt, floors, seed):
+    """MhdCase on `coarse` domain cells (dx = 2^-level) holding an mhd_floor_state under helpers.FLOORS[floors]: asserts the
+    density / pressure floors fire, field-free and field-aligned (vA > c_s) cells are present, and the oracle's level step is
+    finite; returns the case, dt and the oracle's unew"""
+    from helpers import FLOORS, MhdCase, mhd_floor_counts, mhd_floor_state
+    smallr, smallc = FLOORS[floors]
+    c = MhdCase(level, riemann=r1d, riemann2d=r2d, slope_type=st, slope_mag_type=smt, bound=bound, coarse=coarse,
+                boxlen=float(coarse[0]), order=2, seed=3, smallr=smallr, smallc=smallc)
+    ext = c.mesh.extent(level)
+    d0 = mhd_floor_state(ext, seed, smallr, smallc, slab_vt=0.3 if r2d == "hlla" else 0.0)
+    nrho, npr, nfree, nfast = mhd_floor_counts(d0, smallr, smallc)
+    ncell = d0[0].size
+    assert min(nrho, npr) >= 0.02 * ncell and nfree >= 0.05 * ncell and nfast >= 10, (nrho, npr, nfree, nfast)
+    c.init_dense(d0)
+    dt, _ = c.oracle_courant()
+    assert np.isfinite(dt) and dt > 0
+    dt *= 0.7
+    unew = c.oracle_godunov(dt, nthreads=4)
+    assert np.isfinite(unew).all()
+    return c, ext, dt, unew
+
+
+@pytest.mark.parametrize("floors", ["default", "raised"])
+@pytest.mark.parametrize("box", ["cube", "shell"])
+@pytest.mark.parametrize("r1d,r2d,st,smt", MHD_FLOOR_PAIRS)
+def test_mhd_six_pass_kernels_emulated_at_the_floors(orc, dev, floors, box, r1d, r2d, st, smt):
+    """the six MHD passes of mhd_dense.cuh on an mhd_floor_state -- a periodic 16^3 box, and a 24x16x8 box between zero-gradient
+    x ends -- under the RAMSES floors and raised ones: ctoprim's pressure floor, the density / pressure clamps of every traced
+    face and edge state, the field-free sub-box (1-D solvers reduce to hydro, the smallc floor of the 2-D HLLD Alfven speeds) and
+    the field-aligned slab (HLLD's degenerate star state, Roe's bt = 0 branch) are all at work; the owned cells equal set_unew +
+    godunov_fine of the oracle, bit for bit (both copies of every face field)"""
+    from helpers import level_slots
+    coarse, level, bound = ((1, 1, 1), 4, (0,) * 6) if box == "cube" else ((3, 2, 1), 3, (2, 2, 0, 0, 0, 0))
+    c, ext, dt, unew = _mhd_floor_case(coarse, level, bound, r1d, r2d, st, smt, floors, 21 + st)
+    shell = [int(bound[2 * d] > 0) for d in range(3)]
+    uin, act, slot = level_slots(c.mesh, level, c.u, 11)
+    uout = np.zeros_like(uin)
+    dev.devnum_mhd_sweep_box.argtypes = [IP3, IP3, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double),
+                                         C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int]
+    dev.devnum_mhd_sweep_box(IP3(*ext), IP3(*shell), orc.MHD_RIEMANN[r1d], orc.MHD_RIEMANN2D[r2d], 0 if st == 0 else 1,
+                             orc.dptr(uin), orc.dptr(uout), dt, 2.0 ** -level, c.p.gamma, c.p.smallr, c.p.smallc, st, smt)
+    s = c.mesh.s
+    U, U0 = unew.reshape(11, s.ncell), c.u.reshape(11, s.ncell)
+    moved = 0.0
+    for ind in range(8):
+        cells = s.ncoarse + ind * s.ngridmax + act - 1
+        moved = max(moved, float(np.abs(U[:, cells] - U0[:, cells]).max()))
+        assert np.array_equal(uout[:, ind, slot], U[:, cells]), (ind, float(np.abs(uout[:, ind, slot] - U[:, cells]).max()))
+    assert moved > 0
+
+
+def _mhd_box_floor_case(coarse, level, bound, floors, seed):
+    """MhdCase (hlld / hlld, slope_type 1) holding an mhd_floor_state under helpers.FLOORS[floors], with the floors and the
+    degenerate-field cells asserted present; returns the case and the owned extent"""
+    from helpers import FLOORS, MhdCase, mhd_floor_counts, mhd_floor_state
+    smallr, smallc = FLOORS[floors]
+    c = MhdCase(level, riemann="hlld", riemann2d="hlld", slope_type=1, bound=bound, coarse=coarse, boxlen=float(coarse[0]), order=2,
+                seed=3, smallr=smallr, smallc=smallc)
+    ext = c.mesh.extent(level)
+    d0 = mhd_floor_state(ext, seed, smallr, smallc)
+    nrho, npr, nfree, nfast = mhd_floor_counts(d0, smallr, smallc)
+    assert min(nrho, npr) >= 0.02 * d0[0].size and nfree > 0 and nfast > 0, (nrho, npr, nfree, nfast)
+    c.init_dense(d0)
+    return c, ext
+
+
+@pytest.mark.parametrize("floors", ["default", "raised"])
+@pytest.mark.parametrize("coarse,level,bound,nblocks", [((1, 1, 1), 4, (0,) * 6, 3), ((3, 2, 1), 3, (2, 2, 0, 0, 0, 0), 5),
+                                                        ((1, 2, 1), 4, (1, 1, 2, 2, 0, 0), 2)])
+def test_mhd_courant_kernel_emulated_at_the_floors(orc, dev, floors, coarse, level, bound, nblocks):
+    """the stand-alone MHD Courant scan (mhd_courant_kernel: grid-stride loop over the owned cells, cmpdt with its density and
+    pressure floors, warp and block reductions) on mhd_floor_state boxes, periodic or with a wall / outflow shell, under both
+    helpers.FLOORS settings: the reduced time step equals orc_mhd_courant_fine's bit for bit, the mass / energy / internal /
+    magnetic sums agree to 1e-12"""
+    from helpers import level_slots
+    c, ext = _mhd_box_floor_case(coarse, level, bound, floors, 51 + nblocks)
+    dt_ref, sums = c.oracle_courant()
+    assert np.isfinite(dt_ref) and dt_ref > 0 and np.isfinite(sums).all()
+    uin, _, _ = level_slots(c.mesh, level, c.u, 11)
+    shell = [int(bound[2 * d] > 0) for d in range(3)]
+    part = np.zeros(5 * nblocks)
+    dx = 2.0 ** -level
+    dev.devnum_mhd_courant.argtypes = [IP3, IP3, C.c_int, C.POINTER(C.c_double), C.c_double, C.c_double, C.c_double, C.c_double,
+                                       C.c_double, C.POINTER(C.c_double)]
+    dev.devnum_mhd_courant(IP3(*ext), IP3(*shell), nblocks, orc.dptr(np.ascontiguousarray(uin)), dx, c.p.gamma, c.p.smallr,
+                           c.p.smallc, c.p.courant_factor, orc.dptr(part))
+    p5 = part.reshape(5, nblocks)
+    assert min(p5[0].min(), c.p.courant_factor * dx / c.p.smallc, c.p.boxlen / c.p.smallc) == dt_ref
+    got = p5[1:].sum(axis=1) * dx ** 3
+    assert np.all(np.abs(got - sums) <= 1e-12 * np.abs(sums).max()), (got, sums)
+
+
+def _oct_slots(mesh, l):
+    """{oct index: slot} of the active and boundary octs of level l in the dense-box layout of level_slots"""
+    act = mesh.active(l).astype(np.int64)
+    ig = np.concatenate([act] + [mesh.bound(b, l).astype(np.int64) for b in range(mesh.s.nboundary)])
+    pos = mesh._pos_fast(l, ig)
+    q = pos - pos.min(axis=0)
+    no = pos.max(axis=0) - pos.min(axis=0) + 1
+    return dict(zip(ig.tolist(), (q[:, 0] + no[0] * (q[:, 1] + no[1] * q[:, 2])).tolist()))
+
+
+@pytest.mark.parametrize("floors", ["default", "raised"])
+@pytest.mark.parametrize("bound", [(2, 2, 0, 0, 0, 0), (1, 1, 2, 2, 0, 0), (2, 1, 1, 2, 1, 1), (2, 2, 2, 2, 2, 2)])
+def test_mhd_boundary_kernel_emulated_at_the_floors(orc, dev, floors, bound):
+    """make_boundary_hydro of the dense MHD path (mhd_boundary_kernel, one launch per boundary region in the reference's order)
+    on a 16^3 mhd_floor_state between reflexive walls and zero-gradient ends, corner octs included: the ghost octs are scrambled
+    first, then refilled by one pass; the zero-gradient branch removes and restores ekin with the density floored at smallr, which the
+    near-vacuum cells next to the boundary take.  Every ghost oct equals orc_mhd_make_boundary_hydro's, bit for bit."""
+    c, ext = _mhd_box_floor_case((1, 1, 1), 4, bound, floors, 61)
+    m, s, lev = c.mesh, c.mesh.s, 4
+    U = c.u.reshape(11, s.ncell)
+    edge = np.zeros(tuple(ext[::-1]), dtype=bool)
+    for d in range(3):
+        if 2 in bound[2 * d:2 * d + 2]:
+            edge[(slice(None),) * (2 - d) + ([0, -1],)] = True
+    d0 = c.dense()
+    assert (d0[0][edge] < c.p.smallr).sum() > 0                  # floored densities next to a zero-gradient face
+    ghost = []
+    for b in range(s.nboundary):
+        for g in m.bound(b, lev).astype(np.int64):
+            for ind in range(8):
+                ghost.append(s.ncoarse + ind * s.ngridmax + g - 1)
+    ghost = np.array(ghost)
+    U[:, ghost] = 9.0
+    from helpers import level_slots
+    uin, _, _ = level_slots(m, lev, c.u, 11)
+    uin = np.ascontiguousarray(uin)
+    ref = c.u.copy()
+    orc.lib().orc_mhd_make_boundary_hydro(C.byref(c.p), m.ptr, lev, orc.dptr(ref))
+    slots = _oct_slots(m, lev)
+    shell = [int(bound[2 * d] > 0) for d in range(3)]
+    dev.devnum_mhd_boundary.argtypes = [IP3, IP3, C.c_int, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_double), C.c_double]
+    types = m.boundary_types()
+    assert any(t // 10 == 1 for t in types)
+    for b in range(s.nboundary):
+        lst = np.array([slots[g] for g in m.bound(b, lev).astype(np.int64).tolist()], dtype=np.int32)
+        if len(lst):
+            dev.devnum_mhd_boundary(IP3(*ext), IP3(*shell), int(types[b]), orc.iptr(lst), len(lst), orc.dptr(uin), c.p.smallr)
+    R = ref.reshape(11, s.ncell)
+    refilled = ~(R[:, ghost] == 9.0).all(axis=0)      # corner octs that read a not yet refilled neighbour need a second pass
+    assert np.isfinite(R[:, ghost]).all() and refilled.mean() > 0.5
+    for b in range(s.nboundary):
+        for g in m.bound(b, lev).astype(np.int64).tolist():
+            for ind in range(8):
+                got, exp = uin[:, ind, slots[g]], R[:, s.ncoarse + ind * s.ngridmax + g - 1]
+                assert np.array_equal(got, exp), (b, g, ind, got - exp)
+
+
+def _mhd_amr_floor_run(orc, ndim, r1, r2, slope_type, floors, field_scale, seed):
+    """the refined meshes of the MHD AMR tests above (imhd-tube 1-D, Orszag-Tang 2-D, the nested 3-D mesh) with every cell
+    overwritten by fill_mhd_floor_cells; returns the run and its godfine / upload / courant / boundary routines"""
+    from helpers import fill_mhd_floor_cells
+    L = orc.lib()
+    if ndim == 1:
+        from oracle.amr_mhd import MhdAmrRun
+        from test_oracle_golden import IMHD
+        r = MhdAmrRun(5, 9, (2, 2, 0, 0, 0, 0), 3.5, nsubcycle=[1, 1, 1, 1], riemann=r1, slope_type=slope_type, gamma=1.6666667,
+                      courant_factor=0.8, err_grad_d=0.01, err_grad_u=0.05, err_grad_p=0.05, interpol_type=2, regions=IMHD,
+                      tout=[1e9], ngridmax=10000)
+        r.run(max_coarse=10)
+        fns = (L.orc_mhd1_godunov_fine, L.orc_mhd1_upload_fine, L.orc_mhd1_courant_fine, L.orc_mhd1_make_boundary_hydro)
+    elif ndim == 2:
+        from oracle.amr_mhd import MhdAmrRun2D
+        r = MhdAmrRun2D(4, 6, 1.0, nsubcycle=[1], riemann=r1, riemann2d=r2, slope_type=slope_type, gamma=1.6666667,
+                        courant_factor=0.8, err_grad_p=0.1, interpol_type=2, tout=[1e9], nexpand=1, ngridmax=20000)
+        r.run(max_coarse=6)
+        fns = (L.orc_mhd2_godunov_fine, L.orc_mhdn_upload_fine, L.orc_mhdn_courant_fine, None)
+    else:
+        r = _mhd3_static_run(r1, r2, slope_type)
+        fns = (L.orc_mhd3_godunov_fine, L.orc_mhdn_upload_fine, L.orc_mhdn_courant_fine, None)
+    fill_mhd_floor_cells(r, floors, seed, field_scale)
+    # a stable step for the new state: _mhd_amr_compare_levels advances level l by 0.5 dtnew(levelmin) / 2^(l - levelmin)
+    dts = [fns[2](C.byref(r.pm), r.mp, l, r.p.boxlen / r.p.smallc, orc.dptr(r.uold)) * 2.0 ** (l - r.levelmin)
+           for l in range(r.levelmin, r.nlevelmax + 1) if len(r.active[l])]
+    r.dtnew[r.levelmin] = min(dts)
+    return r, fns
+
+
+@pytest.mark.parametrize("ndim,r1,r2,slope_type,field_scale,floors", [
+    (1, "hlld", "llf", 1, 1.0, "default"), (1, "roe", "llf", 2, 1.0, "default"), (1, "hydro", "llf", 1, 0.0, "default"),
+    (1, "hlld", "llf", 1, 1.0, "raised"), (1, "roe", "llf", 2, 1.0, "raised"), (1, "hydro", "llf", 1, 0.0, "raised"),
+    (2, "hlld", "hlld", 2, 1.0, "raised"), (2, "roe", "llf", 1, 1.0, "raised"), (2, "hlld", "hlld", 1, 0.0, "raised"),
+    (2, "llf", "roe", 2, 1.0, "raised"), (3, "hlld", "hlld", 2, 1.0, "raised"), (3, "roe", "roe", 1, 0.0, "raised")])
+def test_mhd_amr_kernels_emulated_at_the_floors(orc, dev, ndim, r1, r2, slope_type, field_scale, floors):
+    """the MHD AMR kernels (mhd_amr.cuh) in 1-D, 2-D and 3-D on refined meshes whose every cell holds floor-state draws
+    (helpers.fill_mhd_floor_cells: densities down to 0.1 smallr, cold magnetised and cold hypersonic cells, magnetically dominated
+    near-vacuum) with the mesh's own divergence-free face fields, or none (field_scale = 0: a field-free tree): ctoprim's
+    floors, the trace resets, prolongation of floored father cells, upload_fine, cmpdt and (1-D) the outflow boundaries equal the
+    oracle bit for bit on every level, refluxed coarse cells included.  (The 2-D and 3-D trees under the RAMSES floors are left
+    out: there the oracle's own update is not finite -- NaN face fields from the corner EMFs of near-vacuum cells.)"""
+    r, (god, upl, cour, bnd) = _mhd_amr_floor_run(orc, ndim, r1, r2, slope_type, floors, field_scale, 31 + ndim)
+    if field_scale == 0:
+        assert (r.uold.reshape(11, -1)[5:] == 0).all()
+    nlev, nrefl, moved = _mhd_amr_compare_levels(orc, dev, r, ndim, r1, r2, slope_type, 2, god, upl, cour, boundary=bnd)
+    assert nlev >= 3 and nrefl > 0 and moved > 0

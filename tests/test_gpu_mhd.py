@@ -238,13 +238,15 @@ def _mhd_commons_from_run(r, ndim, riemann, riemann2d, slope_type):
         a.boundary[l] = [np.array(r.bound[b][l], dtype=np.int32) for b in range(m.nboundary)]
     a.boundary_type = [m.boundary_type[b] for b in range(m.nboundary)]
     a.gamma, a.courant_factor = r.pm.gamma, r.pm.courant_factor
+    a.smallr, a.smallc = r.pm.smallr, r.pm.smallc
     a.slope_type, a.slope_mag_type, a.riemann, a.riemann2d, a.nvector = slope_type, -1, riemann, riemann2d, r.nvector
     return a
 
 
-def _mhd_amr_gpu_vs_oracle(r, ndim, riemann, riemann2d, slope_type, ncoarse, resident, regrid=True):
+def _mhd_amr_gpu_vs_oracle(r, ndim, riemann, riemann2d, slope_type, ncoarse, resident, regrid=True, fill=None):
     """ncoarse coarse steps (with sub-cycling) of the frozen mesh of run `r` on the device -- host-driven amr_step order or the
-    device-resident stepper -- against the oracle's amr_step: every active cell of every level, and dtnew(levelmin)"""
+    device-resident stepper -- against the oracle's amr_step: every active cell of every level, and dtnew(levelmin).
+    fill(r), when given, replaces the state of the frozen mesh first."""
     from ramses_b200.hydro import amr_step
     levelmin, levelmax = r.levelmin, r.nlevelmax
     # regrid once more like the head of amr_step, then freeze the mesh (tests/test_gpu_amr.py::run_case)
@@ -252,6 +254,8 @@ def _mhd_amr_gpu_vs_oracle(r, ndim, riemann, riemann2d, slope_type, ncoarse, res
         if i > levelmin:
             r.make_boundary_hydro(i)
         r.refine_fine(i)
+    if fill is not None:
+        fill(r)
     nlev = [len(r.active[l]) for l in range(1, levelmax + 1)]
     assert sum(1 for n in nlev[levelmin:] if n > 0) >= 1, nlev
     a = _mhd_commons_from_run(r, ndim, riemann, riemann2d, slope_type)
