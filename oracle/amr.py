@@ -21,9 +21,10 @@ class AmrRun:
     def __init__(self, ndim, levelmin, levelmax, bound_type, boxlen, nsubcycle, nexpand=1, ngridmax=2000,
                  riemann="hllc", slope_type=2, gamma=1.4, courant_factor=0.8, err_grad_d=-1.0, err_grad_u=-1.0,
                  err_grad_p=-1.0, interpol_type=1, interpol_var=0, regions=(), tout=(), nvector=32,
-                 floor_d=1e-10, floor_u=1e-10, floor_p=1e-10, bound_regions=None, coarse=(1, 1, 1)):
+                 floor_d=1e-10, floor_u=1e-10, floor_p=1e-10, bound_regions=None, coarse=(1, 1, 1), nvar=None):
         """coarse = (nx, ny, nz) domain coarse cells (orc_mesh_new_box); the mesh-adaptation driver itself is exercised with
-        one domain coarse cell, several are for trees fabricated elsewhere and loaded into son / father / nbor / lists."""
+        one domain coarse cell, several are for trees fabricated elsewhere and loaded into son / father / nbor / lists.
+        nvar = ndim+2 (default) + the number of passive scalars; the initial conditions (regions) leave the scalars at 0."""
         self.ndim, self.levelmin, self.nlevelmax = ndim, levelmin, levelmax
         self.T, self.twondim = 1 << ndim, 2 * ndim
         L = self.L = orc.lib()
@@ -52,8 +53,8 @@ class AmrRun:
         self.nbor = np.ctypeslib.as_array(m.nbor, shape=(2 * ndim, m.ngridmax + 1))
         self.xg = np.ctypeslib.as_array(m.xg, shape=(ndim, m.ngridmax + 1))
         self.p = orc.make_params(ndim=ndim, riemann=riemann, slope_type=slope_type, gamma=gamma,
-                                 courant_factor=courant_factor, boxlen=boxlen, nvector=nvector)
-        self.nvar = ndim + 2
+                                 courant_factor=courant_factor, boxlen=boxlen, nvector=nvector, nvar=nvar)
+        self.nvar = self.p.nvar
         self.uold = np.zeros(self.nvar * m.ncell)
         self.unew = np.zeros(self.nvar * m.ncell)
         self.flag1 = np.zeros(m.ncell + 1, dtype=np.int32)

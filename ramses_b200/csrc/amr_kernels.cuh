@@ -1049,23 +1049,28 @@ __global__ void amr_fill_shell_coupled_kernel(const AmrTree t, const double* __r
     for (int n = 0; n < 5; n++) u[((size_t)n * 8 + is) * nslot + s] = u2[is][n];
 }
 
+// the instantiation of amr_godfine_kernel that runs a (nullptr: none is built for it); launch_amr_godfine launches it, and the
+// host harness (tests/host_numerics) runs the same selection
+using AmrGodfineKernel = void (*)(const AmrSweepArgs);
+template <int NDIM, int RIEMANN>
+AmrGodfineKernel amr_godfine_select(const AmrSweepArgs& a) {
+  if (a.force || a.pfix) {   // source terms: hydro variables only, no difmag (checked by rgpu_init)
+    if (a.nps != 0 || a.difmag > 0.0) return nullptr;
+    return amr_godfine_kernel<NDIM, RIEMANN, false, 0, true>;
+  }
+  if (a.nps == 0) return a.difmag > 0.0 ? amr_godfine_kernel<NDIM, RIEMANN, true> : amr_godfine_kernel<NDIM, RIEMANN, false>;
+  // passive scalars: NDIM=3, up to 2, without difmag (checked by rgpu_init)
+  if (NDIM == 3 && a.nps == 1) return amr_godfine_kernel<NDIM, RIEMANN, false, (NDIM == 3 ? 1 : 0)>;
+  if (NDIM == 3 && a.nps == 2) return amr_godfine_kernel<NDIM, RIEMANN, false, (NDIM == 3 ? 2 : 0)>;
+  return nullptr;
+}
+
 #ifndef RGPU_HOST_NUMERICS   // (tests/host_numerics compiles the __device__ helpers above with g++: no kernel launches there)
 template <int NDIM, int RIEMANN>
 cudaError_t launch_amr_godfine(const AmrSweepArgs& a, cudaStream_t st) {
-  const int nb = (a.nact + AMR_OPB - 1) / AMR_OPB;
-  if (a.force || a.pfix) {   // source terms: hydro variables only, no difmag (checked by rgpu_init)
-    if (a.nps != 0 || a.difmag > 0.0) return cudaErrorInvalidValue;
-    amr_godfine_kernel<NDIM, RIEMANN, false, 0, true><<<nb, AMR_TPO * AMR_OPB, 0, st>>>(a);
-    return cudaGetLastError();
-  }
-  if (a.nps == 0) {
-    if (a.difmag > 0.0) amr_godfine_kernel<NDIM, RIEMANN, true><<<nb, AMR_TPO * AMR_OPB, 0, st>>>(a);
-    else amr_godfine_kernel<NDIM, RIEMANN, false><<<nb, AMR_TPO * AMR_OPB, 0, st>>>(a);
-  } else if (NDIM == 3 && a.nps == 1) {      // passive scalars: NDIM=3, up to 2, without difmag (checked by rgpu_init)
-    amr_godfine_kernel<NDIM, RIEMANN, false, (NDIM == 3 ? 1 : 0)><<<nb, AMR_TPO * AMR_OPB, 0, st>>>(a);
-  } else if (NDIM == 3 && a.nps == 2) {
-    amr_godfine_kernel<NDIM, RIEMANN, false, (NDIM == 3 ? 2 : 0)><<<nb, AMR_TPO * AMR_OPB, 0, st>>>(a);
-  } else return cudaErrorInvalidValue;
+  const AmrGodfineKernel k = amr_godfine_select<NDIM, RIEMANN>(a);
+  if (!k) return cudaErrorInvalidValue;
+  k<<<(a.nact + AMR_OPB - 1) / AMR_OPB, AMR_TPO * AMR_OPB, 0, st>>>(a);
   return cudaGetLastError();
 }
 #endif

@@ -446,9 +446,8 @@ def test_passive_scalars_refined_mesh_bitwise():
     h.download_state(0)
     h.finalize()
     r = AmrRun(3, levelmin, levelmax, (0,) * 6, 1.0, nsubcycle=[1, 2, 2], ngridmax=a.ngridmax, riemann="hllc", slope_type=1,
-               interpol_type=1, tout=[1e9])
-    r.p.nvar = 7; r.nvar = 7
-    r.uold = u0.ravel().copy(); r.unew = np.zeros_like(r.uold)
+               interpol_type=1, tout=[1e9], nvar=7)
+    r.uold[:] = u0.ravel()
     r.son[1:] = a.son; r.father[1:] = a.father; r.nbor[:, 1:] = a.nbor
     for l in range(1, levelmax + 1):
         r.active[l] = [int(g) for g in a.active[l]]
