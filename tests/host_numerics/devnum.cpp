@@ -11,6 +11,7 @@ static double* rgpu_host_dyn_smem = nullptr;   // dynamic shared memory of an em
 #include "sweep_dense4.cuh" // one-barrier form (includes sweep_dense3.cuh)
 #include "sweep_dense3.cuh" // round-2 form of the 3-D dense sweep + the lane-generic solvers (hydro_vec.cuh)
 
+#include <limits>
 #include <pthread.h>
 #include <thread>
 #include <vector>
@@ -60,6 +61,10 @@ static void emulate_serial(Kernel kernel, const Args& a, long long nblocks, int 
       kernel(a);
     }
 }
+
+// a parameter that the kernels behind an entry point do not read: NaN, so that a kernel which did read it gives NaN instead of
+// the oracle's bits
+static const double kNotRead = std::numeric_limits<double>::quiet_NaN();
 
 static Phys make_phys(double gamma, double smallr, double smallc, double slope_theta, double courant_factor, int slope_type,
                       int niter) {   // mirrors rgpu_init (ramses_b200/csrc/rgpu_api.cu)
@@ -130,7 +135,7 @@ extern "C" {
 // n Riemann problems: ql, qr [n][ndim+2] in solver order (rho, u_n, P, u_t1, u_t2), fg [n][ndim+2]
 void devnum_riemann(int ndim, int solver, int n, const double* ql, const double* qr, double* fg, double gamma, double smallr,
                     double smallc, int niter) {
-  const Phys P = make_phys(gamma, smallr, smallc, 1.5, 0.8, 1, niter);
+  const Phys P = make_phys(gamma, smallr, smallc, kNotRead, kNotRead, 1, niter);
   const int nv = ndim + 2;
   for (int i = 0; i < n; i++) {
     if (ndim == 1) riemann_nd<1>(solver, ql + i * nv, qr + i * nv, fg + i * nv, P);
@@ -141,7 +146,7 @@ void devnum_riemann(int ndim, int solver, int n, const double* ql, const double*
 
 // n cells: u [n][ndim+2] conservative -> q [n][ndim+3] (rho, v, P, 1/rho as the kernels keep it is NOT part of q here)
 void devnum_ctoprim(int ndim, int n, const double* u, double* q, double gamma, double smallr, double smallc) {
-  const Phys P = make_phys(gamma, smallr, smallc, 1.5, 0.8, 1, 10);
+  const Phys P = make_phys(gamma, smallr, smallc, kNotRead, kNotRead, 1, 10);
   const int nv = ndim + 2;
   for (int i = 0; i < n; i++) {
     if (ndim == 1) ctoprim<1>(u + i * nv, q + i * nv, P);
@@ -152,7 +157,7 @@ void devnum_ctoprim(int ndim, int n, const double* u, double* q, double gamma, d
 
 // n cells: dt = cmpdt_cell(u, dx)
 void devnum_cmpdt(int ndim, int n, const double* u, double dx, double* dt, double gamma, double smallr, double smallc, double cfl) {
-  const Phys P = make_phys(gamma, smallr, smallc, 1.5, cfl, 1, 10);
+  const Phys P = make_phys(gamma, smallr, smallc, kNotRead, cfl, 1, 10);
   const int nv = ndim + 2;
   for (int i = 0; i < n; i++) {
     double ei;
@@ -164,7 +169,7 @@ void devnum_cmpdt(int ndim, int n, const double* u, double dx, double* dt, doubl
 
 // n limited slopes of (ql, qc, qr) for slope_type 1, 2, 7, 8 (the one-dimensional limiters)
 void devnum_slope(int slope_type, int n, const double* ql, const double* qc, const double* qr, double* dq, double slope_theta) {
-  const Phys P = make_phys(1.4, 1e-10, 1e-10, slope_theta, 0.8, slope_type, 10);
+  const Phys P = make_phys(1.4, 1e-10, 1e-10, slope_theta, kNotRead, slope_type, 10);
   for (int i = 0; i < n; i++) dq[i] = slope_lcr<3, -1>(ql[i], qc[i], qr[i], P);
 }
 
@@ -174,7 +179,7 @@ void devnum_slope(int slope_type, int n, const double* ql, const double* qc, con
 // flux[(ivar + 5*idim)*27 + (i-1) + 3*((j-1) + 3*(k-1))], faces 1..3.  slope_type 3 is not covered (27-point limiter).
 void devnum_unsplit3d(int solver, int slope_type, double slope_theta, const double* uin, double dx, double dt, double* flux,
                       double gamma, double smallr, double smallc, int niter) {
-  const Phys P = make_phys(gamma, smallr, smallc, slope_theta, 0.8, slope_type, niter);
+  const Phys P = make_phys(gamma, smallr, smallc, slope_theta, kNotRead, slope_type, niter);
   static double q[6][6][6][5], rinv[6][6][6], qm[6][6][6][3][5], qp[6][6][6][3][5];
   for (int k = 0; k < 6; k++)
     for (int j = 0; j < 6; j++)
@@ -283,14 +288,14 @@ void devnum_amr_interpol_full(int ndim, int interpol_type, int interpol_var, int
 // the level's own cells and writes the outer-face fluxes rflux [nact][2*ndim][2^(ndim-1)][nvar]
 void devnum_amr_godfine(int ndim, int solver, int ncoarse, int ngridmax, int nx, int ny, int nz, const int* son, const int* father,
                         const int* nbor, const int* active, int nact, int ilevel, const double* uold, double* unew, double* rflux,
-                        double dt, double dx, int interpol_type, int slope_type, double gamma, double smallr, double smallc,
-                        int niter, double difmag) {
+                        double dt, double dx, int interpol_type, int slope_type, double slope_theta, double gamma, double smallr,
+                        double smallc, int niter, double difmag) {
   AmrSweepArgs a;
   std::memset(&a, 0, sizeof a);
   a.t.son = son - 1; a.t.father = father - 1; a.t.nbor = nbor; a.t.ncoarse = ncoarse; a.t.ngridmax = ngridmax;
   a.t.nx = nx; a.t.ny = ny; a.t.nz = nz; a.t.ncell = (long long)ncoarse + (long long)(1 << ndim) * ngridmax;
   a.active = active; a.nact = nact; a.ilevel = ilevel; a.uold = uold; a.unew = unew; a.rflux = rflux;
-  a.P = make_phys(gamma, smallr, smallc, 1.5, 0.8, slope_type, niter);
+  a.P = make_phys(gamma, smallr, smallc, slope_theta, kNotRead, slope_type, niter);
   a.dt = dt; a.dx = dx; a.inv_dx = 1.0 / dx;
   int ex;
   a.dx_pow2 = (std::frexp(dx, &ex) == 0.5) ? 1 : 0;
@@ -316,11 +321,12 @@ void devnum_amr_godfine(int ndim, int solver, int ncoarse, int ngridmax, int nx,
 // rgpu_godunov_fine does in AMR mode).  uold/unew [nvar][ncell], nvar = ndim+2.
 void devnum_amr_godunov(int ndim, int solver, int ncoarse, int ngridmax, int nx, int ny, int nz, const int* son, const int* father,
                         const int* nbor, const int* active, int nact, int ilevel, const double* uold, double* unew, double dt, double dx,
-                        int interpol_type, int slope_type, double gamma, double smallr, double smallc, int niter, int nvector) {
+                        int interpol_type, int slope_type, double slope_theta, double gamma, double smallr, double smallc, int niter,
+                        int nvector) {
   const int nvar = ndim + 2, TW = 2 * ndim, NSF = 1 << (ndim - 1);
   std::vector<double> rflux((size_t)std::max(1, nact) * TW * NSF * nvar, 0.0);
   devnum_amr_godfine(ndim, solver, ncoarse, ngridmax, nx, ny, nz, son, father, nbor, active, nact, ilevel, uold, unew, rflux.data(), dt, dx,
-                     interpol_type, slope_type, gamma, smallr, smallc, niter, 0.0);
+                     interpol_type, slope_type, slope_theta, gamma, smallr, smallc, niter, 0.0);
   std::vector<int> cells, start, srcs, src;
   build_reflux_schedule(ndim, nvector, nact, active, nbor, son, ngridmax, cells, start, srcs, src);
   if (!cells.empty()) {
@@ -337,14 +343,14 @@ void devnum_amr_godunov(int ndim, int solver, int ncoarse, int ngridmax, int nx,
 // unew holds nvar+2 columns when pfix (divu, enew behind the state); rflux [nact][2*ndim][2^(ndim-1)][nvar(+2)]
 void devnum_amr_godfine_src(int ndim, int solver, int ncoarse, int ngridmax, int nx, int ny, int nz, const int* son, const int* father,
                             const int* nbor, const int* active, int nact, int ilevel, const double* uold, double* unew, double* rflux,
-                            double dt, double dx, int interpol_type, int slope_type, double gamma, double smallr, double smallc,
-                            int niter, const double* force, int pfix, int nvector_reflux) {
+                            double dt, double dx, int interpol_type, int slope_type, double slope_theta, double gamma, double smallr,
+                            double smallc, int niter, const double* force, int pfix, int nvector_reflux) {
   AmrSweepArgs a;
   std::memset(&a, 0, sizeof a);
   a.t.son = son - 1; a.t.father = father - 1; a.t.nbor = nbor; a.t.ncoarse = ncoarse; a.t.ngridmax = ngridmax;
   a.t.nx = nx; a.t.ny = ny; a.t.nz = nz; a.t.ncell = (long long)ncoarse + (long long)(1 << ndim) * ngridmax;
   a.active = active; a.nact = nact; a.ilevel = ilevel; a.uold = uold; a.unew = unew; a.rflux = rflux;
-  a.P = make_phys(gamma, smallr, smallc, 1.5, 0.8, slope_type, niter);
+  a.P = make_phys(gamma, smallr, smallc, slope_theta, kNotRead, slope_type, niter);
   a.dt = dt; a.dx = dx; a.inv_dx = 1.0 / dx;
   int ex;
   a.dx_pow2 = (std::frexp(dx, &ex) == 0.5) ? 1 : 0;
@@ -394,7 +400,7 @@ void devnum_amr_src_pass(int kind, int ndim, int ncoarse, int ngridmax, int nx, 
 // n cells: dt = cmpdt_cell(u, dx, sum|g|)
 void devnum_cmpdt_grav(int ndim, int n, const double* u, const double* gsum, double dx, double* dt, double gamma, double smallr,
                        double smallc, double cfl) {
-  const Phys P = make_phys(gamma, smallr, smallc, 1.5, cfl, 1, 10);
+  const Phys P = make_phys(gamma, smallr, smallc, kNotRead, cfl, 1, 10);
   const int nv = ndim + 2;
   for (int i = 0; i < n; i++) {
     double ei;
@@ -407,7 +413,7 @@ void devnum_cmpdt_grav(int ndim, int n, const double* u, const double* gsum, dou
 // n Riemann problems, internal-energy flux fgdnv(nvar+1) only (pressure_fix)
 void devnum_riemann_eflux(int ndim, int solver, int n, const double* ql, const double* qr, double* fe, double gamma, double smallr,
                           double smallc, int niter) {
-  const Phys P = make_phys(gamma, smallr, smallc, 1.5, 0.8, 1, niter);
+  const Phys P = make_phys(gamma, smallr, smallc, kNotRead, kNotRead, 1, niter);
   const int nv = ndim + 2;
   for (int i = 0; i < n; i++) {
     double fg[5];
@@ -424,9 +430,9 @@ void devnum_riemann_eflux(int ndim, int solver, int n, const double* ql, const d
   }
 }
 
-static MPhys make_mphys(double gamma, double smallr, double smallc) {
+static MPhys make_mphys(double gamma, double smallr, double smallc, double slope_theta, double courant_factor) {
   MPhys M;
-  M.gamma = gamma; M.smallr = smallr; M.smallc = smallc; M.slope_theta = 1.5; M.courant_factor = 0.8;
+  M.gamma = gamma; M.smallr = smallr; M.smallc = smallc; M.slope_theta = slope_theta; M.courant_factor = courant_factor;
   M.smallp = smallr * (smallc * smallc) / gamma;
   M.slope_type = 1; M.slope_mag_type = 1;
   return M;
@@ -445,7 +451,7 @@ void devnum_mhd_amr_godunov(int ndim, int ncoarse, int ngridmax, int nx, int ny,
   const int TW = 2 * ndim, NSF = 1 << (ndim - 1);
   std::vector<double> rflux((size_t)std::max(1, nact) * TW * NSF * MNV, 0.0), remf((size_t)std::max(1, nact) * (ndim == 3 ? 81 : 4), 0.0);
   a.active = active; a.nact = nact; a.ilevel = ilevel; a.uold = uold; a.unew = unew; a.rflux = rflux.data(); a.remf = remf.data();
-  a.P = make_mphys(gamma, smallr, smallc);
+  a.P = make_mphys(gamma, smallr, smallc, kNotRead, kNotRead);   // the AMR kernels build slopes 0-2 and no Courant step
   a.P.slope_type = slope_type; a.P.slope_mag_type = slope_mag_type;
   a.dt = dt; a.dx = dx; a.dt_dev = nullptr;
   a.interpol_type = interpol_type; a.interpol_mag_type = interpol_mag_type < 0 ? interpol_type : interpol_mag_type;
@@ -513,8 +519,7 @@ void devnum_mhd_amr_pass(int kind, int ndim, int ncoarse, int ngridmax, int nx, 
   t.son = son - 1; t.father = father - 1; t.nbor = nbor; t.ncoarse = ncoarse; t.ngridmax = ngridmax; t.nx = nx; t.ny = ny; t.nz = nz;
   t.ncell = (long long)ncoarse + (long long)(1 << ndim) * ngridmax;
   const int T = 1 << ndim;
-  MPhys P = make_mphys(gamma, smallr, smallc);
-  P.courant_factor = cfl;
+  const MPhys P = make_mphys(gamma, smallr, smallc, kNotRead, cfl);
   if (kind == 0) {
     for (int pass = 0; pass < 2; pass++)
       for (int b = 0; b < (n * T + 127) / 128; b++)
@@ -543,7 +548,7 @@ void devnum_mhd_amr_pass(int kind, int ndim, int ncoarse, int ngridmax, int nx, 
 
 // n MHD Riemann problems in solver order (rho, P, v_n, B_n, v_t1, B_t1, v_t2, B_t2): fg [n][9]
 void devnum_mhd_riemann(int solver, int n, const double* ql, const double* qr, double* fg, double gamma, double smallr, double smallc) {
-  const MPhys M = make_mphys(gamma, smallr, smallc);
+  const MPhys M = make_mphys(gamma, smallr, smallc, kNotRead, kNotRead);
   for (int i = 0; i < n; i++) {
     real l[8], r[8], f[9];
     for (int k = 0; k < 8; k++) { l[k] = ql[i * 8 + k]; r[k] = qr[i * 8 + k]; }
@@ -562,7 +567,7 @@ void devnum_mhd_riemann(int solver, int n, const double* ql, const double* qr, d
 // n corner EMFs from the four states (qLL, qRL, qLR, qRR) [n][8] in cmp_mag_flx's solver order
 void devnum_mhd_emf(int solver2d, int n, const double* qLL, const double* qRL, const double* qLR, const double* qRR, double* emf,
                     double gamma, double smallr, double smallc) {
-  const MPhys M = make_mphys(gamma, smallr, smallc);
+  const MPhys M = make_mphys(gamma, smallr, smallc, kNotRead, kNotRead);
   for (int i = 0; i < n; i++) {
     real a[8], b[8], c[8], d[8];
     for (int k = 0; k < 8; k++) { a[k] = qLL[i * 8 + k]; b[k] = qRL[i * 8 + k]; c[k] = qLR[i * 8 + k]; d[k] = qRR[i * 8 + k]; }
@@ -583,13 +588,14 @@ void devnum_mhd_emf(int solver2d, int n, const double* qLL, const double* qRL, c
 // of N^3 cells: uin/uout in the device layout [11][8][nslot] (cell_offset of sweep_dense.cuh), N even
 // on a box of n[0] x n[1] x n[2] owned cells, each axis periodic or with a 2-cell ghost shell (box_geom)
 void devnum_mhd_sweep_box(const int* n, const int* shell, int r1d, int r2d, int sl, const double* uin, double* uout, double dt,
-                          double dx, double gamma, double smallr, double smallc, int slope_type, int slope_mag_type) {
+                          double dx, double gamma, double smallr, double smallc, int slope_type, int slope_mag_type, double slope_theta,
+                          double courant_factor) {
   MhdArgs a;
   std::memset(&a, 0, sizeof a);
   a.g = box_geom(3, n, shell);
   const DenseGeom& g = a.g;
   a.uin = uin; a.uout = uout;
-  a.P = make_mphys(gamma, smallr, smallc);
+  a.P = make_mphys(gamma, smallr, smallc, slope_theta, courant_factor);
   a.P.slope_type = slope_type; a.P.slope_mag_type = slope_mag_type;
   a.dt_dev = &dt; a.dx = dx; a.nc = (long long)g.ncx * g.ncy * g.ncz;
   std::vector<double> W((size_t)MW_NCOMP * a.nc, 0.0), part(5 * 64, 0.0);
@@ -615,7 +621,7 @@ struct MhdCourantHost { const double* u; DenseGeom g; MPhys P; double dx; double
 void devnum_mhd_courant(const int* n, const int* shell, int nblocks, const double* u, double dx, double gamma, double smallr,
                         double smallc, double cfl, double* part) {
   MhdCourantHost a;
-  a.u = u; a.g = box_geom(3, n, shell); a.P = make_mphys(gamma, smallr, smallc); a.P.courant_factor = cfl; a.dx = dx; a.part = part;
+  a.u = u; a.g = box_geom(3, n, shell); a.P = make_mphys(gamma, smallr, smallc, kNotRead, cfl); a.dx = dx; a.part = part;
   emulate_launch([](const MhdCourantHost& c) { mhd_courant_kernel(c.u, c.g, c.P, c.dx, c.part); }, a, nblocks, 256);
 }
 
@@ -646,9 +652,10 @@ void devnum_mhd_boundary(const int* n, const int* shell, int bt, const int* slot
 }
 
 void devnum_mhd_sweep(int N, int r1d, int r2d, int sl, const double* uin, double* uout, double dt, double dx, double gamma,
-                      double smallr, double smallc, int slope_type, int slope_mag_type) {
+                      double smallr, double smallc, int slope_type, int slope_mag_type, double slope_theta, double courant_factor) {
   const int n[3] = {N, N, N};
-  devnum_mhd_sweep_box(n, k_no_shell, r1d, r2d, sl, uin, uout, dt, dx, gamma, smallr, smallc, slope_type, slope_mag_type);
+  devnum_mhd_sweep_box(n, k_no_shell, r1d, r2d, sl, uin, uout, dt, dx, gamma, smallr, smallc, slope_type, slope_mag_type, slope_theta,
+                       courant_factor);
 }
 
 // the fused dense-box sweep (sweep_dense_kernel: persistent CTAs of 32 x BY threads, cp.async staging, warp shuffles in x, shared
@@ -656,14 +663,14 @@ void devnum_mhd_sweep(int N, int r1d, int r2d, int sl, const double* uin, double
 // state in the device layout [nvar][2^ndim][nslot]; nblocks persistent CTAs share the work like on the GPU
 // on a box of n[0] x n[1] x n[2] owned cells (1 beyond ndim), each axis periodic or with a 2-cell ghost shell (box_geom)
 int devnum_sweep_dense_box(int ndim, int solver, const int* n, const int* shell, int nblocks, const double* uin, double* uout,
-                           double dt, double dx, int slope_type, double slope_theta, double gamma, double smallr, double smallc,
-                           int niter, double* part, int late) {
+                           double dt, double dx, int slope_type, double slope_theta, double courant_factor, double gamma,
+                           double smallr, double smallc, int niter, double* part, int late) {
   SweepArgs a;
   std::memset(&a, 0, sizeof a);
   a.g = box_geom(ndim, n, shell);
   const DenseGeom& g = a.g;
   a.uin = uin; a.uout = uout;
-  a.P = make_phys(gamma, smallr, smallc, slope_theta, 0.8, slope_type, niter);
+  a.P = make_phys(gamma, smallr, smallc, slope_theta, courant_factor, slope_type, niter);
   a.dt_dev = nullptr; a.dt_val = dt; a.dx = dx; a.inv_dx = 1.0 / dx;
   int ex;
   a.dx_pow2 = (std::frexp(dx, &ex) == 0.5) ? 1 : 0;
@@ -692,24 +699,24 @@ int devnum_sweep_dense_box(int ndim, int solver, const int* n, const int* shell,
 }
 
 int devnum_sweep_dense(int ndim, int solver, int N, int nblocks, const double* uin, double* uout, double dt, double dx,
-                        int slope_type, double slope_theta, double gamma, double smallr, double smallc, int niter, double* part,
-                        int late) {
+                        int slope_type, double slope_theta, double courant_factor, double gamma, double smallr, double smallc, int niter,
+                        double* part, int late) {
   const int n[3] = {N, ndim > 1 ? N : 1, ndim > 2 ? N : 1};
-  return devnum_sweep_dense_box(ndim, solver, n, k_no_shell, nblocks, uin, uout, dt, dx, slope_type, slope_theta, gamma, smallr,
-                                smallc, niter, part, late);
+  return devnum_sweep_dense_box(ndim, solver, n, k_no_shell, nblocks, uin, uout, dt, dx, slope_type, slope_theta, courant_factor, gamma,
+                                smallr, smallc, niter, part, late);
 }
 
 // the AMR variant of the dense sweep (AMRV=true: fluxes through faces of refined cells reset to zero, the update ACCUMULATES into
 // uout which already holds unew) on a fully refined periodic level of N^3 cells; refined[8][nslot] = son(cell)>0
 void devnum_sweep_dense_amr_box(int solver, const int* n, const int* shell, int nblocks, const double* uin, double* uout,
-                                const unsigned char* refined, double dt, double dx, int slope_type, double gamma, double smallr,
-                                double smallc, int niter) {
+                                const unsigned char* refined, double dt, double dx, int slope_type, double slope_theta, double gamma,
+                                double smallr, double smallc, int niter) {
   SweepArgs a;
   std::memset(&a, 0, sizeof a);
   a.g = box_geom(3, n, shell);
   const DenseGeom& g = a.g;
   a.uin = uin; a.uout = uout; a.refined = refined;
-  a.P = make_phys(gamma, smallr, smallc, 1.5, 0.8, slope_type, niter);
+  a.P = make_phys(gamma, smallr, smallc, slope_theta, kNotRead, slope_type, niter);   // part = NULL: no Courant partials
   a.dt_dev = nullptr; a.dt_val = dt; a.dx = dx; a.inv_dx = 1.0 / dx;
   int ex;
   a.dx_pow2 = (std::frexp(dx, &ex) == 0.5) ? 1 : 0;
@@ -723,9 +730,10 @@ void devnum_sweep_dense_amr_box(int solver, const int* n, const int* shell, int 
 }
 
 void devnum_sweep_dense_amr(int solver, int N, int nblocks, const double* uin, double* uout, const unsigned char* refined, double dt,
-                            double dx, int slope_type, double gamma, double smallr, double smallc, int niter) {
+                            double dx, int slope_type, double slope_theta, double gamma, double smallr, double smallc, int niter) {
   const int n[3] = {N, N, N};
-  devnum_sweep_dense_amr_box(solver, n, k_no_shell, nblocks, uin, uout, refined, dt, dx, slope_type, gamma, smallr, smallc, niter);
+  devnum_sweep_dense_amr_box(solver, n, k_no_shell, nblocks, uin, uout, refined, dt, dx, slope_type, slope_theta, gamma, smallr, smallc,
+                             niter);
 }
 
 
@@ -733,7 +741,7 @@ void devnum_sweep_dense_amr(int solver, int N, int nblocks, const double* uin, d
 // and (b) the 3-lane form riemann_v<R,V3> (problems i, i+1, i+2 in lanes a, b, c; n must be a multiple of 3)
 void devnum_riemann_vec(int solver, int n, const double* ql, const double* qr, double* fg_scalar, double* fg_v3, double gamma,
                         double smallr, double smallc, int niter) {
-  const Phys P = make_phys(gamma, smallr, smallc, 1.5, 0.8, 1, niter);
+  const Phys P = make_phys(gamma, smallr, smallc, kNotRead, kNotRead, 1, niter);
   auto run1 = [&](const double* l, const double* r, double* f) {
     switch (solver) {
       case RIEMANN_LLF: riemann_v<RIEMANN_LLF, double>(l, r, f, P); break;
@@ -767,14 +775,14 @@ void devnum_riemann_vec(int solver, int n, const double* ql, const double* qr, d
 // sweep3_kernel (sweep_dense3.cuh) on a periodic box of N^3 cells, emulated launch; by in {8, 12, 16}, vec in {0, 1, 2}
 // on a box of n[0] x n[1] x n[2] owned cells, each axis periodic or with a 2-cell ghost shell (box_geom)
 int devnum_sweep3_box(int solver, const int* n, const int* shell, int nblocks, const double* uin, double* uout, double dt, double dx,
-                      int slope_type, double slope_theta, double gamma, double smallr, double smallc, int niter, double* part, int by,
-                      int vec) {
+                      int slope_type, double slope_theta, double courant_factor, double gamma, double smallr, double smallc, int niter,
+                      double* part, int by, int vec) {
   SweepArgs a;
   std::memset(&a, 0, sizeof a);
   a.g = box_geom(3, n, shell);
   const DenseGeom& g = a.g;
   a.uin = uin; a.uout = uout;
-  a.P = make_phys(gamma, smallr, smallc, slope_theta, 0.8, slope_type, niter);
+  a.P = make_phys(gamma, smallr, smallc, slope_theta, courant_factor, slope_type, niter);
   a.dt_dev = nullptr; a.dt_val = dt; a.dx = dx; a.inv_dx = 1.0 / dx;
   int ex;
   a.dx_pow2 = (std::frexp(dx, &ex) == 0.5) ? 1 : 0;
@@ -797,15 +805,15 @@ int devnum_sweep3_box(int solver, const int* n, const int* shell, int nblocks, c
 }
 
 int devnum_sweep3(int solver, int N, int nblocks, const double* uin, double* uout, double dt, double dx, int slope_type,
-                  double slope_theta, double gamma, double smallr, double smallc, int niter, double* part, int by, int vec) {
+                  double slope_theta, double courant_factor, double gamma, double smallr, double smallc, int niter, double* part, int by,
+                  int vec) {
   const int n[3] = {N, N, N};
-  return devnum_sweep3_box(solver, n, k_no_shell, nblocks, uin, uout, dt, dx, slope_type, slope_theta, gamma, smallr, smallc, niter,
-                           part, by, vec);
+  return devnum_sweep3_box(solver, n, k_no_shell, nblocks, uin, uout, dt, dx, slope_type, slope_theta, courant_factor, gamma, smallr,
+                           smallc, niter, part, by, vec);
 }
 
 void devnum_mhd_cmpdt(int n, const double* u, double dx, double* dt, double gamma, double smallr, double smallc, double cfl) {
-  MPhys M = make_mphys(gamma, smallr, smallc);
-  M.courant_factor = cfl;
+  const MPhys M = make_mphys(gamma, smallr, smallc, kNotRead, cfl);
   for (int i = 0; i < n; i++) {
     real uu[11];
     for (int k = 0; k < 11; k++) uu[k] = u[i * 11 + k];

@@ -11,13 +11,14 @@ extern "C" {
 // gravity term of the Courant partials (rgpu_level_steps); refined != NULL: the 3-D AMR variant (uout holds unew on entry)
 int devnum_sweep_dense_grav_box(int ndim, int solver, const int* n, const int* shell, int nblocks, const double* uin, double* uout,
                                 const double* force, int gsrc, const unsigned char* refined, double dt, double dx, int slope_type,
-                                double slope_theta, double gamma, double smallr, double smallc, int niter, double* part) {
+                                double slope_theta, double courant_factor, double gamma, double smallr, double smallc, int niter,
+                                double* part) {
   SweepArgs a;
   std::memset(&a, 0, sizeof a);
   a.g = box_geom(ndim, n, shell);
   const DenseGeom& g = a.g;
   a.uin = uin; a.uout = uout; a.force = force; a.gsrc = gsrc; a.refined = refined;
-  a.P = make_phys(gamma, smallr, smallc, slope_theta, 0.8, slope_type, niter);
+  a.P = make_phys(gamma, smallr, smallc, slope_theta, courant_factor, slope_type, niter);
   a.dt_dev = nullptr; a.dt_val = dt; a.dx = dx; a.inv_dx = 1.0 / dx;
   int ex;
   a.dx_pow2 = (std::frexp(dx, &ex) == 0.5) ? 1 : 0;

@@ -49,7 +49,7 @@ extern "C" {
 // fg [n][5+nx], fe [n] the internal-energy flux fgdnv(nvar+1)
 int devnum_riemann_nx(int solver, int nx, int n, const double* ql, const double* qr, double* fg, double* fe, double gamma,
                       double smallr, double smallc, int niter) {
-  const Phys P = make_phys(gamma, smallr, smallc, 1.5, 0.8, 1, niter);
+  const Phys P = make_phys(gamma, smallr, smallc, kNotRead, kNotRead, 1, niter);
   if (nx == 1) riemann_nx_rows<1>(solver, n, ql, qr, fg, fe, P);
   else if (nx == 2) riemann_nx_rows<2>(solver, n, ql, qr, fg, fe, P);
   else return -1;
@@ -60,13 +60,13 @@ int devnum_riemann_nx(int solver, int nx, int n, const double* ql, const double*
 // launch_amr_godfine launches (amr_godfine_select); rflux [nact][2*ndim][2^(ndim-1)][nvar].  Returns -1 when none is built.
 int devnum_amr_godfine_nps(int ndim, int solver, int ncoarse, int ngridmax, int nx, int ny, int nz, const int* son, const int* father,
                            const int* nbor, const int* active, int nact, int ilevel, const double* uold, double* unew, double* rflux,
-                           double dt, double dx, int interpol_type, int interpol_var, int slope_type, double gamma, double smallr,
-                           double smallc, int niter, int nvar) {
+                           double dt, double dx, int interpol_type, int interpol_var, int slope_type, double slope_theta, double gamma,
+                           double smallr, double smallc, int niter, int nvar) {
   AmrSweepArgs a;
   std::memset(&a, 0, sizeof a);
   a.t = make_tree(ndim, ncoarse, ngridmax, nx, ny, nz, son, father, nbor);
   a.active = active; a.nact = nact; a.ilevel = ilevel; a.uold = uold; a.unew = unew; a.rflux = rflux;
-  a.P = make_phys(gamma, smallr, smallc, 1.5, 0.8, slope_type, niter);
+  a.P = make_phys(gamma, smallr, smallc, slope_theta, kNotRead, slope_type, niter);
   a.dt = dt; a.dx = dx; a.inv_dx = 1.0 / dx;
   int ex;
   a.dx_pow2 = (std::frexp(dx, &ex) == 0.5) ? 1 : 0;
@@ -83,13 +83,14 @@ int devnum_amr_godfine_nps(int ndim, int solver, int ncoarse, int ngridmax, int 
 // (amr_schedules.h), as rgpu_godunov_fine does in AMR mode.  uold / unew [nvar][ncell].
 int devnum_amr_godunov_nps(int ndim, int solver, int ncoarse, int ngridmax, int nx, int ny, int nz, const int* son, const int* father,
                            const int* nbor, const int* active, int nact, int ilevel, const double* uold, double* unew, double dt,
-                           double dx, int interpol_type, int interpol_var, int slope_type, double gamma, double smallr, double smallc,
-                           int niter, int nvar, int nvector) {
+                           double dx, int interpol_type, int interpol_var, int slope_type, double slope_theta, double gamma,
+                           double smallr, double smallc, int niter, int nvar, int nvector) {
   const int TW = 2 * ndim, NSF = 1 << (ndim - 1);
   // room for 7 columns whatever nvar is: a kernel of the wrong NPS then gives wrong numbers instead of writing past the buffer
   std::vector<double> rflux((size_t)std::max(1, nact) * TW * NSF * std::max(nvar, 7), 0.0);
   const int rc = devnum_amr_godfine_nps(ndim, solver, ncoarse, ngridmax, nx, ny, nz, son, father, nbor, active, nact, ilevel, uold, unew,
-                                        rflux.data(), dt, dx, interpol_type, interpol_var, slope_type, gamma, smallr, smallc, niter, nvar);
+                                        rflux.data(), dt, dx, interpol_type, interpol_var, slope_type, slope_theta, gamma, smallr, smallc,
+                                        niter, nvar);
   if (rc) return rc;
   std::vector<int> cells, start, srcs, src;
   build_reflux_schedule(ndim, nvector, nact, active, nbor, son, ngridmax, cells, start, srcs, src);

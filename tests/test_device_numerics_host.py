@@ -40,9 +40,9 @@ def dev():
     L.devnum_amr_getnborfather.argtypes = [C.c_int] * 6 + [ip, ip, ip, C.c_int, ip, C.c_int, ip]
     L.devnum_amr_interpol.argtypes = [C.c_int, C.c_int, C.c_int, dp, dp]
     L.devnum_amr_godfine.argtypes = [C.c_int] * 7 + [ip, ip, ip, ip, C.c_int, C.c_int, dp, dp, dp, C.c_double, C.c_double, C.c_int,
-                                     C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, C.c_double]
+                                     C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_double]
     L.devnum_amr_godfine_src.argtypes = [C.c_int] * 7 + [ip, ip, ip, ip, C.c_int, C.c_int, dp, dp, dp, C.c_double, C.c_double, C.c_int,
-                                         C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, dp, C.c_int, C.c_int]
+                                         C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, dp, C.c_int, C.c_int]
     L.devnum_amr_src_pass.argtypes = [C.c_int] * 7 + [ip, ip, ip, ip, C.c_int, dp, dp, dp, dp, dp] + [C.c_double] * 5
     L.devnum_cmpdt_grav.argtypes = [C.c_int, C.c_int, dp, dp, C.c_double, dp, C.c_double, C.c_double, C.c_double, C.c_double]
     L.devnum_riemann_eflux.argtypes = [C.c_int, C.c_int, C.c_int, dp, dp, dp, C.c_double, C.c_double, C.c_double, C.c_int]
@@ -50,12 +50,14 @@ def dev():
         [C.c_double] * 3 + [C.c_int]
     L.devnum_mhd_amr_pass.argtypes = [C.c_int] * 7 + [ip, ip, ip, ip, C.c_int, dp] + [C.c_double] * 5 + [C.c_int, C.c_int, dp]
     i3 = C.c_int * 3
-    L.devnum_sweep3_box.argtypes = [C.c_int, i3, i3, C.c_int, dp, dp] + [C.c_double] * 2 + [C.c_int] + [C.c_double] * 4 + \
+    L.devnum_sweep3_box.argtypes = [C.c_int, i3, i3, C.c_int, dp, dp] + [C.c_double] * 2 + [C.c_int] + [C.c_double] * 5 + \
         [C.c_int, dp, C.c_int, C.c_int]
     L.devnum_sweep_dense_box.argtypes = [C.c_int, C.c_int, i3, i3, C.c_int, dp, dp] + [C.c_double] * 2 + [C.c_int] + \
-        [C.c_double] * 4 + [C.c_int, dp, C.c_int]
+        [C.c_double] * 5 + [C.c_int, dp, C.c_int]
     L.devnum_sweep_dense_amr_box.argtypes = [C.c_int, i3, i3, C.c_int, dp, dp, C.POINTER(C.c_ubyte)] + [C.c_double] * 2 + \
-        [C.c_int] + [C.c_double] * 3 + [C.c_int]
+        [C.c_int] + [C.c_double] * 4 + [C.c_int]
+    L.devnum_mhd_sweep_box.argtypes = [i3, i3, C.c_int, C.c_int, C.c_int, dp, dp] + [C.c_double] * 5 + [C.c_int, C.c_int] + \
+        [C.c_double] * 2
     return L
 
 
@@ -782,7 +784,7 @@ def _amr_oct_batch_compare(orc, dev, ndim, solver, difmag, floors=None):
         rflux = np.zeros(len(act) * 2 * ndim * (T // 2) * nvar)
         dev.devnum_amr_godfine(ndim, sid, r.ncoarse, r.ngridmax, m.nx, m.ny, m.nz, orc.iptr(son), orc.iptr(father), orc.iptr(nbor),
                                orc.iptr(act), len(act), l, orc.dptr(r.uold), orc.dptr(unew_k), orc.dptr(rflux), dt, dx, itype, st,
-                               1.4, r.p.smallr, r.p.smallc, 10, difmag)
+                               r.p.slope_theta, 1.4, r.p.smallr, r.p.smallc, 10, difmag)
         assert np.isfinite(unew_o).all()
         Uo, Uk = unew_o.reshape(nvar, r.ncell), unew_k.reshape(nvar, r.ncell)
         for ind in range(T):
@@ -816,11 +818,15 @@ def test_amr_source_terms_emulated_at_the_floors(orc, dev, floors, ndim, solver,
     _amr_source_terms_compare(orc, dev, ndim, solver, grav, pfix, floors)
 
 
-def _amr_source_terms_compare(orc, dev, ndim, solver, grav, pfix, floors=None):
+def _amr_source_terms_compare(orc, dev, ndim, solver, grav, pfix, floors=None, run=None, beta_fix=0.5):
     """the body of test_amr_source_terms_emulated_on_the_cpu_equal_oracle; floors: a floor_state on every cell, under
-    helpers.FLOORS[floors]"""
+    helpers.FLOORS[floors]; run: a developed AMR run (interpolation type 2 below 3-D, 1 in 3-D) used instead of the meshes above,
+    with its slope_type, gamma, slope_theta, niter_riemann and boxlen.  Returns (cells where the energy switch fired, cells
+    compared)."""
     from oracle.amr import FastAmrRun
-    if ndim == 1:
+    if run is not None:
+        r, itype, st = run, (2 if ndim < 3 else 1), run.p.slope_type
+    elif ndim == 1:
         reg = [dict(type="square", x_center=0.25, length_x=0.5, d=1.0, p=1.0), dict(type="square", x_center=0.75, length_x=0.5, d=0.125, p=0.1)]
         r = FastAmrRun(1, 3, 8, (1, 1, 0, 0, 0, 0), 1.0, nsubcycle=[1, 2], ngridmax=500, riemann=solver, slope_type=2,
                        err_grad_d=0.05, err_grad_p=0.05, interpol_type=2, regions=reg, tout=[1e9])
@@ -837,7 +843,8 @@ def _amr_source_terms_compare(orc, dev, ndim, solver, grav, pfix, floors=None):
         r = FastAmrRun(3, 3, 5, (0,) * 6, 1.0, nsubcycle=[1, 2], ngridmax=4000, riemann=solver, slope_type=1, err_grad_p=0.1,
                        interpol_type=1, regions=reg, tout=[1e9])
         itype, st = 1, 1
-    r.run(max_coarse=3)
+    if run is None:
+        r.run(max_coarse=3)
     dt_floor = _put_floor_state(r, ndim, floors, 50 + ndim) if floors else None
     m = r.m
     T, nvar, nc = 1 << ndim, ndim + 2, r.ncell
@@ -851,8 +858,7 @@ def _amr_source_terms_compare(orc, dev, ndim, solver, grav, pfix, floors=None):
     rng = np.random.default_rng(7 * ndim + sid)
     # an arbitrary acceleration field (f is an input of the path): a uniform pull plus cell-to-cell structure, strong enough to matter
     force = np.ascontiguousarray((np.array([0.7, -0.4, 0.3])[:ndim, None] + 0.3 * rng.standard_normal((ndim, nc))) * 5.0)
-    beta_fix = 0.5
-    nlev, switched, gmoved, dmax, nrefl = 0, 0, 0.0, 0.0, 0
+    nlev, switched, gmoved, dmax, nrefl, ncmp = 0, 0, 0.0, 0.0, 0, 0
     try:
         for l in range(r.levelmin, r.nlevelmax + 1):
             act = np.ascontiguousarray(r.active[l], dtype=np.int32)
@@ -884,13 +890,14 @@ def _amr_source_terms_compare(orc, dev, ndim, solver, grav, pfix, floors=None):
             if pfix:
                 divu_k[:] = 7.0; enew_k[:] = -3.0
             args = (ndim, r.ncoarse, r.ngridmax, m.nx, m.ny, m.nz, orc.iptr(son), orc.iptr(father), orc.iptr(nbor), orc.iptr(act), len(act))
-            tail = (orc.dptr(force), 1.4, r.p.smallr, beta_fix, dx, dt)
+            tail = (orc.dptr(force), r.p.gamma, r.p.smallr, beta_fix, dx, dt)
             if pfix:
                 dev.devnum_amr_src_pass(0, *args, orc.dptr(uold_k), orc.dptr(unew_k), orc.dptr(divu_k), orc.dptr(enew_k), *tail)
             rflux = np.zeros(len(act) * 2 * ndim * (T // 2) * ncol)
             dev.devnum_amr_godfine_src(ndim, sid, r.ncoarse, r.ngridmax, m.nx, m.ny, m.nz, orc.iptr(son), orc.iptr(father), orc.iptr(nbor),
                                        orc.iptr(act), len(act), l, orc.dptr(uold_k), orc.dptr(unew_k), orc.dptr(rflux), dt, dx, itype, st,
-                                       1.4, r.p.smallr, r.p.smallc, 10, orc.dptr(force) if grav else None, 1 if pfix else 0, r.nvector)
+                                       r.p.slope_theta, r.p.gamma, r.p.smallr, r.p.smallc, r.p.niter_riemann,
+                                       orc.dptr(force) if grav else None, 1 if pfix else 0, r.nvector)
             # after the sweep and the coarse reflux pass, before the sources: the WHOLE arrays -- the level's own cells and the coarser
             # cells that received refluxes (state, and with pressure_fix divu / enew, which reflux like two more variables)
             assert np.array_equal(unew_k[: nvar * nc], unew_mid), l
@@ -913,14 +920,16 @@ def _amr_source_terms_compare(orc, dev, ndim, solver, grav, pfix, floors=None):
             got, ref = uold_k.reshape(nvar, nc)[:, cells], uold_o.reshape(nvar, nc)[:, cells]
             assert np.array_equal(got, ref), (l, np.abs(got - ref).max())
             gmoved = max(gmoved, float(np.abs(ref - before).max()))
+            ncmp += len(cells)
             nlev += 1
     finally:
         L.orc_set_pressure_fix(None, None, 0.0)
         L.orc_set_gravity(None)
     assert nlev >= 3 and gmoved > 1e-6 and (dmax > 0 or not pfix) and nrefl > 0
-    if pfix and (ndim == 3 or floors):
+    if pfix and (ndim == 3 or floors) and beta_fix > 0:
         assert switched > 0          # the cold Sedov background (p = 1e-5) and the cold hypersonic cells trip the energy switch
     assert np.isfinite(uold_o).all()
+    return switched, ncmp
 
 
 MHD_R1D = {"llf": 0, "roe": 1, "hll": 2, "hlld": 3, "upwind": 4, "hydro": 5}
@@ -1164,7 +1173,7 @@ def test_mhd_six_pass_kernels_emulated_on_the_cpu_equal_oracle(orc, dev, r1d, r2
     from helpers import MhdCase, mhd_smooth_state
     dp = C.POINTER(C.c_double)
     dev.devnum_mhd_sweep.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, dp, dp, C.c_double, C.c_double, C.c_double, C.c_double,
-                                     C.c_double, C.c_int, C.c_int]
+                                     C.c_double, C.c_int, C.c_int, C.c_double, C.c_double]
     N, level = 16, 4
     c = MhdCase(level, riemann=r1d, riemann2d=r2d, slope_type=st)
     d0 = mhd_smooth_state(N)
@@ -1176,7 +1185,7 @@ def test_mhd_six_pass_kernels_emulated_on_the_cpu_equal_oracle(orc, dev, r1d, r2
     uout = np.zeros_like(uin)
     sl = 0 if st == 0 else 1
     dev.devnum_mhd_sweep(N, orc.MHD_RIEMANN[r1d], orc.MHD_RIEMANN2D[r2d], sl, orc.dptr(np.ascontiguousarray(uin)), orc.dptr(uout),
-                         dt, 1.0 / N, c.p.gamma, c.p.smallr, c.p.smallc, st, st)
+                         dt, 1.0 / N, c.p.gamma, c.p.smallr, c.p.smallc, st, st, c.p.slope_theta, c.p.courant_factor)
     got = uout[:, ind.ravel(), slot.ravel()].reshape(11, N, N, N)
     assert np.abs(ref - c.dense()).max() > 1e-4
     assert np.array_equal(got, ref)
@@ -1214,7 +1223,7 @@ def test_dense_sweep_kernel_emulated_on_the_cpu_equals_oracle(orc, dev, ndim, so
     variant of the plane loop (template parameter LATE, not dispatched by the product yet) gives the same bits."""
     dp = C.POINTER(C.c_double)
     dev.devnum_sweep_dense.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, dp, dp, C.c_double, C.c_double, C.c_int, C.c_double,
-                                       C.c_double, C.c_double, C.c_double, C.c_int, dp, C.c_int]
+                                       C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, dp, C.c_int]
     from helpers import Case, smooth_state
     level = int(np.log2(N))
     c = Case(ndim, level, riemann=solver, slope_type=st, slope_theta=1.3)
@@ -1230,8 +1239,8 @@ def test_dense_sweep_kernel_emulated_on_the_cpu_equals_oracle(orc, dev, ndim, so
     uout = np.zeros_like(uin)
     part = np.zeros(4 * 64)
     sid = {"llf": 0, "exact": 1, "acoustic": 2, "hllc": 3, "hll": 4}[solver]
-    nb = dev.devnum_sweep_dense(ndim, sid, N, nblocks, orc.dptr(np.ascontiguousarray(uin)), orc.dptr(uout), dt, 1.0 / N, st, 1.3, 1.4,
-                                1e-10, 1e-10, 10, orc.dptr(part), late)
+    nb = dev.devnum_sweep_dense(ndim, sid, N, nblocks, orc.dptr(np.ascontiguousarray(uin)), orc.dptr(uout), dt, 1.0 / N, st, 1.3, 0.8,
+                                1.4, 1e-10, 1e-10, 10, orc.dptr(part), late)
     got = uout[:, ind.ravel(), slot.ravel()].reshape(ref.shape)
     assert np.abs(ref - c.dense()).max() > 1e-4
     assert np.array_equal(got, ref)
@@ -1249,7 +1258,7 @@ def test_dense_sweep_amr_variant_emulated_on_the_cpu_equals_oracle(orc, dev, sol
     from oracle.amr import FastAmrRun
     dp = C.POINTER(C.c_double)
     dev.devnum_sweep_dense_amr.argtypes = [C.c_int, C.c_int, C.c_int, dp, dp, C.POINTER(C.c_ubyte), C.c_double, C.c_double, C.c_int,
-                                           C.c_double, C.c_double, C.c_double, C.c_int]
+                                           C.c_double, C.c_double, C.c_double, C.c_double, C.c_int]
     reg = [dict(type="square", x_center=0.5, y_center=0.5, z_center=0.5, length_x=10, length_y=10, length_z=10, exp_region=10, d=1.0, p=1e-5),
            dict(type="point", x_center=0.5, y_center=0.5, z_center=0.5, p=0.4)]
     r = FastAmrRun(3, 4, 5, (0,) * 6, 1.0, nsubcycle=[1, 2], ngridmax=6000, riemann=solver, slope_type=1, err_grad_p=0.1,
@@ -1286,7 +1295,7 @@ def test_dense_sweep_amr_variant_emulated_on_the_cpu_equals_oracle(orc, dev, sol
     sid = {"llf": 0, "exact": 1, "acoustic": 2, "hllc": 3, "hll": 4}[solver]
     uout = np.ascontiguousarray(uout)
     dev.devnum_sweep_dense_amr(sid, N, 4, orc.dptr(np.ascontiguousarray(uin)), orc.dptr(uout),
-                               np.ascontiguousarray(refined).ctypes.data_as(C.POINTER(C.c_ubyte)), dt, 1.0 / N, 1, 1.4, 1e-10, 1e-10, 10)
+                               np.ascontiguousarray(refined).ctypes.data_as(C.POINTER(C.c_ubyte)), dt, 1.0 / N, 1, 1.5, 1.4, 1e-10, 1e-10, 10)
     assert np.abs(ref - uin).max() > 1e-5
     assert np.array_equal(uout, ref)
 
@@ -1325,7 +1334,7 @@ def test_sweep3_kernel_emulated_on_the_cpu_equals_oracle(orc, dev, solver, st, N
     solver forms 0 (branching scalar), 1 (3-lane), 2 (branch-free scalar)."""
     dp = C.POINTER(C.c_double)
     dev.devnum_sweep3.argtypes = [C.c_int, C.c_int, C.c_int, dp, dp, C.c_double, C.c_double, C.c_int, C.c_double, C.c_double,
-                                  C.c_double, C.c_double, C.c_int, dp, C.c_int, C.c_int]
+                                  C.c_double, C.c_double, C.c_double, C.c_int, dp, C.c_int, C.c_int]
     from helpers import Case, smooth_state
     level = int(np.log2(N))
     c = Case(3, level, riemann=solver, slope_type=st, slope_theta=1.3)
@@ -1341,8 +1350,8 @@ def test_sweep3_kernel_emulated_on_the_cpu_equals_oracle(orc, dev, solver, st, N
     uout = np.zeros_like(uin)
     part = np.zeros(4 * 64)
     sid = {"llf": 0, "exact": 1, "acoustic": 2, "hllc": 3, "hll": 4}[solver]
-    nb = dev.devnum_sweep3(sid, N, nblocks, orc.dptr(np.ascontiguousarray(uin)), orc.dptr(uout), dt, 1.0 / N, st, 1.3, 1.4,
-                           1e-10, 1e-10, 10, orc.dptr(part), by, vec)
+    nb = dev.devnum_sweep3(sid, N, nblocks, orc.dptr(np.ascontiguousarray(uin)), orc.dptr(uout), dt, 1.0 / N, st, 1.3, 0.8,
+                           1.4, 1e-10, 1e-10, 10, orc.dptr(part), by, vec)
     got = uout[:, ind.ravel(), slot.ravel()].reshape(ref.shape)
     assert np.abs(ref - c.dense()).max() > 1e-4
     assert np.array_equal(got, ref)
@@ -1409,7 +1418,7 @@ def test_sweep3_kernel_emulated_on_non_cubic_boxes(orc, dev, coarse, level, boun
     on boxes with a ghost shell on one axis only: the owned cells equal one level step of the oracle bit for bit, and the fused
     Courant partials give the oracle's next time step.  nblocks never divides the work count."""
     dev.devnum_sweep3_box.argtypes = [C.c_int, IP3, IP3, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_double,
-                                      C.c_double, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int,
+                                      C.c_double, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int,
                                       C.POINTER(C.c_double), C.c_int, C.c_int]
     from helpers import level_slots
     c, ext, dt, unew = _box_case(3, level, coarse, bound, solver, st)
@@ -1418,7 +1427,7 @@ def test_sweep3_kernel_emulated_on_non_cubic_boxes(orc, dev, coarse, level, boun
     uout = np.zeros_like(uin)
     part = np.zeros(4 * 64)
     nb = dev.devnum_sweep3_box(SOLVER_ID[solver], IP3(*ext), IP3(*shell), nblocks, orc.dptr(uin), orc.dptr(uout), dt,
-                               2.0 ** -level, st, 1.3, 1.4, 1e-10, 1e-10, 10, orc.dptr(part), by, vec)
+                               2.0 ** -level, st, 1.3, 0.8, 1.4, 1e-10, 1e-10, 10, orc.dptr(part), by, vec)
     ntx, nty = -(-ext[0] // 30), -(-ext[1] // (by - 2))
     assert nb == nblocks and (ntx * nty * ext[2]) % nblocks != 0
     _check_box_result(c, uout, act, slot, unew, part, nb, 3)
@@ -1439,8 +1448,8 @@ def test_dense_sweep_kernel_emulated_on_non_cubic_boxes(orc, dev, ndim, coarse, 
     """sweep_dense_kernel (1-D, 2-D and 3-D forms) on boxes of several coarse cells with different extents per axis, periodic or
     with a ghost shell on one axis: the owned cells equal one level step of the oracle bit for bit."""
     dev.devnum_sweep_dense_box.argtypes = [C.c_int, C.c_int, IP3, IP3, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double),
-                                           C.c_double, C.c_double, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int,
-                                           C.POINTER(C.c_double), C.c_int]
+                                           C.c_double, C.c_double, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double,
+                                           C.c_int, C.POINTER(C.c_double), C.c_int]
     from helpers import level_slots
     c, ext, dt, unew = _box_case(ndim, level, coarse, bound, solver, st)
     shell = [int(bound[2 * d] > 0) for d in range(3)]
@@ -1448,7 +1457,7 @@ def test_dense_sweep_kernel_emulated_on_non_cubic_boxes(orc, dev, ndim, coarse, 
     uout = np.zeros_like(uin)
     part = np.zeros(4 * 64)
     nb = dev.devnum_sweep_dense_box(ndim, SOLVER_ID[solver], IP3(*ext), IP3(*shell), nblocks, orc.dptr(uin), orc.dptr(uout), dt,
-                                    2.0 ** -level, st, 1.3, 1.4, 1e-10, 1e-10, 10, orc.dptr(part), 0)
+                                    2.0 ** -level, st, 1.3, 0.8, 1.4, 1e-10, 1e-10, 10, orc.dptr(part), 0)
     _check_box_result(c, uout, act, slot, unew, part, nb, ndim)
 
 
@@ -1465,8 +1474,6 @@ def test_mhd_six_pass_kernels_emulated_on_non_cubic_boxes(orc, dev, coarse, leve
     cells with different extents per axis, periodic or between zero-gradient x ends: the owned cells equal set_unew + godunov_fine
     of the oracle, bit for bit (both copies of every face field)."""
     from helpers import MhdCase, level_slots, mhd_box_state
-    dev.devnum_mhd_sweep_box.argtypes = [IP3, IP3, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double),
-                                         C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int]
     c = MhdCase(level, riemann=r1d, riemann2d=r2d, slope_type=st, bound=bound, coarse=coarse, boxlen=float(coarse[0]), order=2,
                 seed=3)
     ext = c.mesh.extent(level)
@@ -1480,7 +1487,8 @@ def test_mhd_six_pass_kernels_emulated_on_non_cubic_boxes(orc, dev, coarse, leve
     uin, act, slot = level_slots(c.mesh, level, c.u, 11)
     uout = np.zeros_like(uin)
     dev.devnum_mhd_sweep_box(IP3(*ext), IP3(*shell), orc.MHD_RIEMANN[r1d], orc.MHD_RIEMANN2D[r2d], 0 if st == 0 else 1,
-                             orc.dptr(uin), orc.dptr(uout), dt, 2.0 ** -level, c.p.gamma, c.p.smallr, c.p.smallc, st, st)
+                             orc.dptr(uin), orc.dptr(uout), dt, 2.0 ** -level, c.p.gamma, c.p.smallr, c.p.smallc, st, st,
+                             c.p.slope_theta, c.p.courant_factor)
     _check_box_result(c, uout, act, slot, unew, None, 0, 3)
 
 
@@ -1539,7 +1547,7 @@ def _dense_amr_box_compare(orc, dev, coarse, bound, solver, nblocks, floors=None
     smallr, smallc = FLOORS[floors] if floors else (1e-10, 1e-10)
     dev.devnum_sweep_dense_amr_box.argtypes = [C.c_int, IP3, IP3, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double),
                                                C.POINTER(C.c_ubyte), C.c_double, C.c_double, C.c_int, C.c_double, C.c_double,
-                                               C.c_double, C.c_int]
+                                               C.c_double, C.c_double, C.c_int]
     lev = 4
     c = Case(3, lev, riemann=solver, slope_type=1, bound=bound, coarse=coarse, boxlen=float(coarse[0]), order=2, seed=8,
              smallr=smallr, smallc=smallc)
@@ -1573,7 +1581,7 @@ def _dense_amr_box_compare(orc, dev, coarse, bound, solver, nblocks, floors=None
     unmasked = uout.copy()
     for mask, out in ((refined, uout), (np.zeros_like(refined), unmasked)):
         dev.devnum_sweep_dense_amr_box(SOLVER_ID[solver], IP3(*ext), IP3(*shell), nblocks, orc.dptr(uin), orc.dptr(out),
-                                       mask.ctypes.data_as(C.POINTER(C.c_ubyte)), dt, 2.0 ** -lev, 1, 1.4, smallr, smallc, 10)
+                                       mask.ctypes.data_as(C.POINTER(C.c_ubyte)), dt, 2.0 ** -lev, 1, 1.5, 1.4, smallr, smallc, 10)
     assert not np.array_equal(unmasked, uout)              # the marks matter
     assert np.isfinite(unew).all()
     Un, Us = unew.reshape(5, s.ncell), start.reshape(5, s.ncell)
@@ -1623,7 +1631,7 @@ def test_sweep3_kernel_emulated_at_the_floors(orc, dev, floors, solver, st, nblo
     uout = np.zeros_like(uin)
     part = np.zeros(4 * 64)
     nb = dev.devnum_sweep3_box(SOLVER_ID[solver], IP3(*ext), IP3(0, 0, 0), nblocks, orc.dptr(uin), orc.dptr(uout), dt,
-                               2.0 ** -c.level, st, 1.3, 1.4, c.p.smallr, c.p.smallc, 10, orc.dptr(part), by, vec)
+                               2.0 ** -c.level, st, 1.3, 0.8, 1.4, c.p.smallr, c.p.smallc, 10, orc.dptr(part), by, vec)
     _check_box_result(c, uout, act, slot, unew, part, nb, 3)
 
 
@@ -1648,7 +1656,7 @@ def test_dense_sweep_kernel_emulated_at_the_floors(orc, dev, floors, ndim, ext, 
     uout = np.zeros_like(uin)
     part = np.zeros(4 * 64)
     nb = dev.devnum_sweep_dense_box(ndim, SOLVER_ID[solver], IP3(*ext), IP3(*shell), nblocks, orc.dptr(uin), orc.dptr(uout), dt,
-                                    2.0 ** -c.level, st, 1.3, 1.4, c.p.smallr, c.p.smallc, 10, orc.dptr(part), 0)
+                                    2.0 ** -c.level, st, 1.3, 0.8, 1.4, c.p.smallr, c.p.smallc, 10, orc.dptr(part), 0)
     _check_box_result(c, uout, act, slot, unew, part, nb, ndim)
 
 
@@ -1703,10 +1711,9 @@ def test_mhd_six_pass_kernels_emulated_at_the_floors(orc, dev, floors, box, r1d,
     shell = [int(bound[2 * d] > 0) for d in range(3)]
     uin, act, slot = level_slots(c.mesh, level, c.u, 11)
     uout = np.zeros_like(uin)
-    dev.devnum_mhd_sweep_box.argtypes = [IP3, IP3, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double),
-                                         C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int]
     dev.devnum_mhd_sweep_box(IP3(*ext), IP3(*shell), orc.MHD_RIEMANN[r1d], orc.MHD_RIEMANN2D[r2d], 0 if st == 0 else 1,
-                             orc.dptr(uin), orc.dptr(uout), dt, 2.0 ** -level, c.p.gamma, c.p.smallr, c.p.smallc, st, smt)
+                             orc.dptr(uin), orc.dptr(uout), dt, 2.0 ** -level, c.p.gamma, c.p.smallr, c.p.smallc, st, smt,
+                             c.p.slope_theta, c.p.courant_factor)
     s = c.mesh.s
     U, U0 = unew.reshape(11, s.ncell), c.u.reshape(11, s.ncell)
     moved = 0.0

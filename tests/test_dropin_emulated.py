@@ -40,7 +40,7 @@ def attach_emulated_hydro(r, orc, dev, riemann, slope_type, interpol_type):
         dims, (son, father, nbor) = _tree(r)
         dx = 0.5 ** l * r.p.boxlen / (r.m.icoarse_max - r.m.icoarse_min + 1)
         dev.devnum_amr_godunov(r.ndim, HYD[riemann], *dims, orc.iptr(son), orc.iptr(father), orc.iptr(nbor), orc.iptr(act), len(act), l,
-                               orc.dptr(r.uold), orc.dptr(r.unew), r.dtnew[l], dx, interpol_type, slope_type, r.p.gamma, r.p.smallr,
+                               orc.dptr(r.uold), orc.dptr(r.unew), r.dtnew[l], dx, interpol_type, slope_type, r.p.slope_theta, r.p.gamma, r.p.smallr,
                                r.p.smallc, 10, r.nvector)
         calls[0] += 1
     r.c_godunov_fine = c_godunov_fine
@@ -68,7 +68,7 @@ def attach_emulated_mhd(r, orc, dev, ndim, riemann, riemann2d, slope_type, inter
 def _argtypes(dev):
     ip, dp = C.POINTER(C.c_int), C.POINTER(C.c_double)
     dev.devnum_amr_godunov.argtypes = [C.c_int] * 7 + [ip, ip, ip, ip, C.c_int, C.c_int, dp, dp, C.c_double, C.c_double, C.c_int, C.c_int,
-                                       C.c_double, C.c_double, C.c_double, C.c_int, C.c_int]
+                                       C.c_double, C.c_double, C.c_double, C.c_double, C.c_int, C.c_int]
 
 
 def _same_run(a, b):

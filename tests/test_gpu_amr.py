@@ -26,6 +26,7 @@ def commons_from_run(r, riemann, slope_type):
     a.boundary_type = [m.boundary_type[b] for b in range(m.nboundary)]
     a.gamma, a.courant_factor = r.p.gamma, r.p.courant_factor
     a.slope_type, a.riemann, a.nvector = slope_type, riemann, r.nvector
+    a.slope_theta, a.niter_riemann = r.p.slope_theta, r.p.niter_riemann
     a.difmag = r.p.difmag
     a.smallr, a.smallc = r.p.smallr, r.p.smallc
     return a
@@ -71,16 +72,18 @@ BOUND_2D_WALLS_X_OUTFLOW_Y = [(1, (0, 0), (1, 1), (0, 0)), (2, (2, 2), (1, 1), (
 
 def run_case(ndim, levelmin, levelmax, bound, regions, riemann, slope_type, ncoarse_dev, interpol_type, nsub, boxlen=1.0,
              err=0.05, nexpand=1, difmag=0.0, bound_regions=None, interpol_var=0, gravity=False, pressure_fix=False, beta_fix=0.5,
-             device_resident=False, floors=None):
-    """one coarse step of an adaptively refined mesh, developed by the oracle's regridding driver and then frozen, on the GPU
-    (host-driven amr_step order, or rgpu_amr_steps) and on the oracle; floors: every cell then holds a floor_state cell under
-    helpers.FLOORS[floors] (helpers.fill_floor_state) for the compared step"""
+             device_resident=False, floors=None, gamma=1.4, courant_factor=0.8, slope_theta=1.5, niter_riemann=10, ncoarse=1):
+    """ncoarse coarse steps (one by default) of an adaptively refined mesh, developed by the oracle's regridding driver and then
+    frozen, on the GPU (host-driven amr_step order, or rgpu_amr_steps) and on the oracle; floors: every cell then holds a
+    floor_state cell under helpers.FLOORS[floors] (helpers.fill_floor_state) for the compared steps"""
     from oracle.amr import AmrRun
     from ramses_b200.hydro import HydroGPU
     r = AmrRun(ndim, levelmin, levelmax, bound, boxlen, nsubcycle=nsub, nexpand=nexpand, ngridmax=20000, riemann=riemann,
                slope_type=slope_type, err_grad_d=err, err_grad_u=err, err_grad_p=err, interpol_type=interpol_type,
-               interpol_var=interpol_var, regions=regions, tout=[1e9], bound_regions=bound_regions)
+               interpol_var=interpol_var, regions=regions, tout=[1e9], bound_regions=bound_regions, gamma=gamma,
+               courant_factor=courant_factor)
     r.p.difmag = difmag                            # hydro_parameters.f90:81 (cmpdivu + consup in unsplit)
+    r.p.slope_theta, r.p.niter_riemann = slope_theta, niter_riemann
     r.flag_coarse(); r.init_refine(); r.init_refine_2()
     for _ in range(ncoarse_dev):                   # develop the flow with the full (regridding) driver
         r.refine_coarse(); r.push_lists(1)
@@ -127,12 +130,14 @@ def run_case(ndim, levelmin, levelmax, bound, regions, riemann, slope_type, ncoa
     dtold = {l: r.dtold[l] for l in range(0, levelmax + 2)}
     if device_resident:      # rgpu_amr_steps: dtnew / dtold stay on the device, the source passes read dt from there
         a.numbtot = {l: len(a.active[l]) for l in range(1, levelmax + 1)}
-        dts = h.amr_steps(levelmin, [0] + [r.nsubcycle[l] for l in range(1, levelmax + 1)], 1)
-        dtnew[levelmin] = dts[0]
+        dts = h.amr_steps(levelmin, [0] + [r.nsubcycle[l] for l in range(1, levelmax + 1)], ncoarse)
+        dtnew[levelmin] = dts[-1]
     else:
-        gpu_amr_step(h, a, r, levelmin, 1, dtnew, dtold)
+        for _ in range(ncoarse):
+            gpu_amr_step(h, a, r, levelmin, 1, dtnew, dtold)
     h.download_state(0)
     extra = h.download_pressure_fix() if pressure_fix else None
+    r.dev_info = {l: h.level_info(l) for l in range(1, levelmax + 1) if len(a.active[l])}   # which kernel swept each level
     h.finalize()
     # oracle: the same coarse step on the frozen mesh
     r.static = True
@@ -149,7 +154,8 @@ def run_case(ndim, levelmin, levelmax, bound, regions, riemann, slope_type, ncoa
             L.orc_set_pressure_fix(orc.dptr(divu_o), orc.dptr(enew_o), beta_fix)
         if gravity:
             L.orc_set_gravity(orc.dptr(force))
-        r.amr_step(levelmin, 1)
+        for _ in range(ncoarse):
+            r.amr_step(levelmin, 1)
     finally:
         L.orc_set_pressure_fix(None, None, 0.0)
         L.orc_set_gravity(None)

@@ -239,6 +239,7 @@ def _mhd_commons_from_run(r, ndim, riemann, riemann2d, slope_type):
     a.boundary_type = [m.boundary_type[b] for b in range(m.nboundary)]
     a.gamma, a.courant_factor = r.pm.gamma, r.pm.courant_factor
     a.smallr, a.smallc = r.pm.smallr, r.pm.smallc
+    a.slope_theta = r.pm.slope_theta
     a.slope_type, a.slope_mag_type, a.riemann, a.riemann2d, a.nvector = slope_type, -1, riemann, riemann2d, r.nvector
     return a
 

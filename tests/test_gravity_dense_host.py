@@ -30,7 +30,7 @@ def grav_dev():
     L.devnum_sweep_dense_grav_box.restype = C.c_int
     L.devnum_sweep_dense_grav_box.argtypes = [C.c_int, C.c_int, IP3, IP3, C.c_int, DP, DP, DP, C.c_int, C.POINTER(C.c_ubyte),
                                               C.c_double, C.c_double, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double,
-                                              C.c_int, DP]
+                                              C.c_double, C.c_int, DP]
     return L
 
 
@@ -103,7 +103,7 @@ def test_gravity_dense_sweep_emulated_equals_oracle(orc, grav_dev, ndim, coarse,
     uout = np.zeros_like(uin)
     part = np.zeros(4 * 64)
     nb = grav_dev.devnum_sweep_dense_grav_box(ndim, SOLVER_ID[solver], IP3(*ext), IP3(*shell), nblocks, orc.dptr(uin), orc.dptr(uout),
-                                              orc.dptr(fin), gsrc, None, dt, 2.0 ** -level, st, 1.3, 1.4, 1e-10, 1e-10, 10,
+                                              orc.dptr(fin), gsrc, None, dt, 2.0 ** -level, st, 1.3, 0.8, 1.4, 1e-10, 1e-10, 10,
                                               orc.dptr(part))
     T = 1 << ndim
     U, Ung = unew.reshape(ndim + 2, s.ncell), unew_nograv.reshape(ndim + 2, s.ncell)
@@ -176,7 +176,7 @@ def test_gravity_dense_sweep_amr_variant_emulated_equals_oracle(orc, grav_dev, c
     shell = [int(bound[2 * d] > 0) for d in range(3)]
     grav_dev.devnum_sweep_dense_grav_box(3, SOLVER_ID[solver], IP3(*ext), IP3(*shell), nblocks, orc.dptr(uin), orc.dptr(uout),
                                          orc.dptr(fin), 0, refined.ctypes.data_as(C.POINTER(C.c_ubyte)), dt, 2.0 ** -lev, 1, 1.5,
-                                         1.4, 1e-10, 1e-10, 10, None)
+                                         0.8, 1.4, 1e-10, 1e-10, 10, None)
     Un = unew.reshape(5, s.ncell)
     for ind in range(8):
         cc = s.ncoarse + ind * s.ngridmax + act - 1
@@ -213,7 +213,7 @@ def test_gravity_dense_sweep_emulated_at_the_floors(orc, grav_dev, floors, ndim,
     uout = np.zeros_like(uin)
     part = np.zeros(4 * 64)
     nb = grav_dev.devnum_sweep_dense_grav_box(ndim, SOLVER_ID[solver], IP3(*c.mesh.extent(level)), IP3(0, 0, 0), nblocks, orc.dptr(uin),
-                                              orc.dptr(uout), orc.dptr(fin), 1, None, dt, 2.0 ** -level, st, 1.3, 1.4, smallr, smallc, 10,
+                                              orc.dptr(uout), orc.dptr(fin), 1, None, dt, 2.0 ** -level, st, 1.3, 0.8, 1.4, smallr, smallc, 10,
                                               orc.dptr(part))
     U = unew.reshape(ndim + 2, s.ncell)
     for ind in range(1 << ndim):

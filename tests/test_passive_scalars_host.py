@@ -35,9 +35,9 @@ def scl():
     L = C.CDLL(lib, mode=os.RTLD_LOCAL | os.RTLD_NOW)
     L.devnum_riemann_nx.argtypes = [C.c_int, C.c_int, C.c_int, DP, DP, DP, DP, C.c_double, C.c_double, C.c_double, C.c_int]
     L.devnum_amr_godfine_nps.argtypes = [C.c_int] * 7 + [IP, IP, IP, IP, C.c_int, C.c_int, DP, DP, DP, C.c_double, C.c_double] + \
-        [C.c_int] * 3 + [C.c_double] * 3 + [C.c_int, C.c_int]
+        [C.c_int] * 3 + [C.c_double] * 4 + [C.c_int, C.c_int]
     L.devnum_amr_godunov_nps.argtypes = [C.c_int] * 7 + [IP, IP, IP, IP, C.c_int, C.c_int, DP, DP, C.c_double, C.c_double] + \
-        [C.c_int] * 3 + [C.c_double] * 3 + [C.c_int] * 3
+        [C.c_int] * 3 + [C.c_double] * 4 + [C.c_int] * 3
     L.devnum_amr_list_pass.argtypes = [C.c_int] * 7 + [IP, IP, IP, IP, C.c_int, C.c_int, DP, DP, C.c_double, C.c_int, C.c_int, DP]
     return L
 
@@ -181,10 +181,15 @@ def test_amr_oct_batch_kernel_with_scalars_equals_oracle(orc, scl, sedov_runs, s
         r.uold[:] = uold
 
 
-def _godfine_compare(orc, scl, r, solver, st, itype, ivar, nvar, dt_of=None):
+def _godfine_compare(orc, scl, r, solver, st, itype, ivar, nvar, dt_of=None, params=None):
+    """params: gamma, slope_theta, niter_riemann and the box scale (boxlen of the one coarse cell) of both sides, instead of the
+    defaults; returns the oracle's unew of every level"""
     dims, (son, father, nbor) = _tree_args(r)
     L = orc.lib()
-    p = orc.make_params(ndim=3, nvar=nvar, riemann=solver, slope_type=st, nvector=r.nvector, smallr=r.p.smallr, smallc=r.p.smallc)
+    q = params or dict(gamma=1.4, slope_theta=1.5, niter_riemann=10, scale=1.0)
+    p = orc.make_params(ndim=3, nvar=nvar, riemann=solver, slope_type=st, nvector=r.nvector, smallr=r.p.smallr, smallc=r.p.smallc,
+                        gamma=q["gamma"], slope_theta=q["slope_theta"], niter_riemann=q["niter_riemann"], boxlen=q["scale"])
+    refs = []
     nlev, moved = 0, 0.0
     T, nc = 8, r.ncell
     try:
@@ -194,10 +199,11 @@ def _godfine_compare(orc, scl, r, solver, st, itype, ivar, nvar, dt_of=None):
             if len(act) == 0:
                 continue
             dt = dt_of(l) if dt_of else 0.4 * r.dtnew[r.levelmin] / 2 ** (l - r.levelmin)
-            dx = 0.5 ** l
+            dx = q["scale"] * 0.5 ** l
             unew_o = np.zeros_like(r.uold)
             L.orc_set_unew(C.byref(p), r.mp, l, orc.dptr(r.uold), orc.dptr(unew_o))
             L.orc_godunov_fine(C.byref(p), r.mp, l, dt, orc.dptr(r.uold), orc.dptr(unew_o), 1)
+            refs.append(unew_o)
             # uold / unew with NaN columns up to 7 variables behind the state: a kernel built for the wrong NPS (a broken selection)
             # reads and writes them and fails the comparison, instead of running past the arrays
             pad = np.full((7 - nvar) * nc, np.nan) if nvar < 7 else np.zeros(0)
@@ -205,8 +211,8 @@ def _godfine_compare(orc, scl, r, solver, st, itype, ivar, nvar, dt_of=None):
             unew_k = np.concatenate([np.zeros_like(r.uold), pad])
             L.orc_set_unew(C.byref(p), r.mp, l, orc.dptr(r.uold), orc.dptr(unew_k))
             assert scl.devnum_amr_godunov_nps(3, SOLVER_ID[solver], *dims, orc.iptr(son), orc.iptr(father), orc.iptr(nbor), orc.iptr(act),
-                                              len(act), l, orc.dptr(uold_k), orc.dptr(unew_k), dt, dx, itype, ivar, st, 1.4, r.p.smallr,
-                                              r.p.smallc, 10, nvar, r.nvector) == 0
+                                              len(act), l, orc.dptr(uold_k), orc.dptr(unew_k), dt, dx, itype, ivar, st, q["slope_theta"], q["gamma"],
+                                              r.p.smallr, r.p.smallc, q["niter_riemann"], nvar, r.nvector) == 0
             unew_k = unew_k[:nvar * nc]
             assert np.isfinite(unew_o).all()
             assert np.array_equal(unew_k, unew_o), (l, float(np.abs(unew_k - unew_o).max()))
@@ -217,6 +223,7 @@ def _godfine_compare(orc, scl, r, solver, st, itype, ivar, nvar, dt_of=None):
     finally:
         _set_interpol(orc, 1, 0)
     assert nlev >= 3 and moved > 1e-6
+    return tuple(refs)
 
 
 def test_amr_oct_batch_kernel_selection_rejects_what_is_not_built(orc, scl, sedov_runs):
@@ -228,9 +235,9 @@ def test_amr_oct_batch_kernel_selection_rejects_what_is_not_built(orc, scl, sedo
     u = np.zeros(8 * r.ncell)
     rf = np.zeros(len(act) * 6 * 4 * 8)
     assert scl.devnum_amr_godfine_nps(3, 3, *dims, orc.iptr(son), orc.iptr(father), orc.iptr(nbor), orc.iptr(act), len(act), 3,
-                                      orc.dptr(u), orc.dptr(u.copy()), orc.dptr(rf), 1e-3, 0.125, 1, 0, 1, 1.4, 1e-10, 1e-10, 10, 8) == -1
+                                      orc.dptr(u), orc.dptr(u.copy()), orc.dptr(rf), 1e-3, 0.125, 1, 0, 1, 1.5, 1.4, 1e-10, 1e-10, 10, 8) == -1
     assert scl.devnum_amr_godfine_nps(2, 3, *dims, orc.iptr(son), orc.iptr(father), orc.iptr(nbor), orc.iptr(act), len(act), 3,
-                                      orc.dptr(u), orc.dptr(u.copy()), orc.dptr(rf), 1e-3, 0.125, 1, 0, 1, 1.4, 1e-10, 1e-10, 10, 5) == -1
+                                      orc.dptr(u), orc.dptr(u.copy()), orc.dptr(rf), 1e-3, 0.125, 1, 0, 1, 1.5, 1.4, 1e-10, 1e-10, 10, 5) == -1
 
 
 # ---- floor states: the oct-batch kernel and the set_uold floor fix ------------------------------------------------------------
@@ -270,7 +277,7 @@ def test_scalar_floor_fix_at_the_floors_equals_oracle(orc, scl, sedov_runs, floo
             uold_k, unew_k = r.uold.copy(), np.zeros_like(r.uold)
             L.orc_set_unew(C.byref(p), r.mp, l, orc.dptr(uold_k), orc.dptr(unew_k))
             assert scl.devnum_amr_godunov_nps(3, SOLVER_ID[solver], *dims, orc.iptr(son), orc.iptr(father), orc.iptr(nbor), orc.iptr(act),
-                                              len(act), l, orc.dptr(uold_k), orc.dptr(unew_k), dt, 0.5 ** l, 1, 0, 2, 1.4, smallr, smallc,
+                                              len(act), l, orc.dptr(uold_k), orc.dptr(unew_k), dt, 0.5 ** l, 1, 0, 2, r.p.slope_theta, 1.4, smallr, smallc,
                                               10, nvar, r.nvector) == 0
             do, dn = uold_k.reshape(nvar, -1)[0, cells], unew_k.reshape(nvar, -1)[0, cells]
             up += int(((do < smallr) & (dn > do)).sum())
@@ -408,7 +415,7 @@ def test_dropin_with_scalars_device_code_equals_oracle(orc, scl, nvar):
                     return
                 dims, (son, father, nbor) = _tree_args(r)
                 assert scl.devnum_amr_godunov_nps(3, SOLVER_ID["hllc"], *dims, orc.iptr(son), orc.iptr(father), orc.iptr(nbor), orc.iptr(act),
-                                                  len(act), l, orc.dptr(r.uold), orc.dptr(r.unew), r.dtnew[l], 0.5 ** l, 1, 0, 2, r.p.gamma,
+                                                  len(act), l, orc.dptr(r.uold), orc.dptr(r.unew), r.dtnew[l], 0.5 ** l, 1, 0, 2, r.p.slope_theta, r.p.gamma,
                                                   r.p.smallr, r.p.smallc, 10, nvar, r.nvector) == 0
                 calls[0] += 1
             r.c_godunov_fine = c_godunov_fine
