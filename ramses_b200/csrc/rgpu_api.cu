@@ -1423,7 +1423,8 @@ int rgpu_bind_tree(int ncoarse, int ngridmax, const int* son, const int* father,
   G.ncoarse = ncoarse; G.ngridmax = ngridmax; G.son = son; G.father = father; G.nbor = nbor;
   if (G.amr) {   // mirror the tree (read-only during a step; re-bind after every regrid)
     const long long ncell = (long long)ncoarse + (long long)T_() * ngridmax;
-    if (ncell != G.ncell) {
+    const bool resized = ncell != G.ncell;
+    if (resized) {
       cudaFree(G.d_son_base); cudaFree(G.d_father); cudaFree(G.d_nbor); cudaFree(G.d_uold); cudaFree(G.d_unew); cudaFree(G.d_force);
       G.d_son_base = nullptr; G.d_son = G.d_father = G.d_nbor = nullptr; G.d_uold = G.d_unew = nullptr; G.d_force = nullptr;
       // one leading zero: son(0) = 0 is what a missing neighbour father cell (nbor == 0 at an uncovered box corner) reads
@@ -1442,9 +1443,22 @@ int rgpu_bind_tree(int ncoarse, int ngridmax, const int* son, const int* father,
       }
       G.ncell = ncell;
     }
-    CUDA_OK(cudaMemcpy(G.d_son, son, sizeof(int) * ncell, cudaMemcpyHostToDevice));
-    CUDA_OK(cudaMemcpy(G.d_father, father, sizeof(int) * ngridmax, cudaMemcpyHostToDevice));
-    CUDA_OK(cudaMemcpy(G.d_nbor, nbor, sizeof(int) * (size_t)2 * G.p.ndim * ngridmax, cudaMemcpyHostToDevice));
+    // on the library's stream: after the kernels that still read the old tree, before the mask kernels below
+    CUDA_OK(cudaMemcpyAsync(G.d_son, son, sizeof(int) * ncell, cudaMemcpyHostToDevice, G.stream));
+    CUDA_OK(cudaMemcpyAsync(G.d_father, father, sizeof(int) * ngridmax, cudaMemcpyHostToDevice, G.stream));
+    CUDA_OK(cudaMemcpyAsync(G.d_nbor, nbor, sizeof(int) * (size_t)2 * G.p.ndim * ngridmax, cudaMemcpyHostToDevice, G.stream));
+    // the refined-cell mask of a dense AMR level is son(cell) > 0 of the level's own cells.  refine_fine(l) changes those sons
+    // without changing level l's lists, so a level bound before its own refine_fine (the reference order: build_comm(l) runs
+    // before refine_fine(l)) or never re-bound (a base level whose octs stay the same) would keep the mask of an older mesh.
+    // A level bound against a tree of another size is skipped: its slots may name octs beyond ngridmax; it must be re-bound
+    for (int l = 1; l <= MAXLEVEL && !resized; l++) {
+      Level& L = G.lev[l];
+      if (!G.alev[l].bound || !G.alev[l].dense_sweep || !L.d_refined) continue;
+      amr_refined_mask_kernel<<<(unsigned)((L.nslot + 255) / 256), 256, 0, G.stream>>>(G.d_son, L.d_refined, L.d_slot_igrid, L.nslot, G.ncoarse,
+                                                                                     G.ngridmax, T_());
+      CUDA_OK(cudaGetLastError());
+    }
+    CUDA_OK(cudaStreamSynchronize(G.stream));
   }
   return RGPU_OK;
 }
