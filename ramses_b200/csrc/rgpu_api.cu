@@ -58,6 +58,11 @@ DECL(2, 0, false) DECL(2, 1, false) DECL(2, 2, false) DECL(2, 3, false) DECL(2, 
 DECL(3, 0, false) DECL(3, 1, false) DECL(3, 2, false) DECL(3, 3, false) DECL(3, 4, false)
 DECL(3, 0, true) DECL(3, 1, true) DECL(3, 2, true) DECL(3, 3, true) DECL(3, 4, true)
 #undef DECL
+// pressure_fix: the PFIX instantiations of the 3-D AMR variant, without and with poisson (sweep_pfix_inst_3d_*.cu)
+#define DECL(R, GRAV) extern template cudaError_t launch_sweep_dense_pfix<R, GRAV>(const SweepArgs&, int, cudaStream_t);
+DECL(0, false) DECL(1, false) DECL(2, false) DECL(3, false) DECL(4, false)
+DECL(0, true) DECL(1, true) DECL(2, true) DECL(3, true) DECL(4, true)
+#undef DECL
 }  // namespace rgpu
 
 using namespace rgpu;
@@ -141,6 +146,7 @@ struct Level {
   double* d_mhdw = nullptr;          // MHD work arrays [MW_NCOMP][ncell_box]
   unsigned char* d_refined = nullptr;  // AMR mode: son(cell)>0 per box cell [2^ndim][nslot]
   double* d_f = nullptr;             // poisson: the acceleration f [ndim][2^ndim][nslot] (rgpu_upload_force; AMR mode: gathered per call)
+  double* d_pfix = nullptr;          // pressure_fix, AMR mode: divu and enew [2][2^ndim][nslot] (gathered from / scattered to d_unew per call)
   bool f_valid = false;              // poisson, levelmin=levelmax: f uploaded since the bind
   double dt_last = 0.0;              // dt of the last godunov_fine (rgpu_set_uold's gravity source term needs it)
   int mhd_nb = 0;                    // CTAs of the MHD update kernel
@@ -564,7 +570,7 @@ void free_level(Level& L) {
   for (auto e : L.ev_c) cudaEventDestroy(e);
   cudaFree(L.d_slot_igrid); cudaFree(L.d_mirror); cudaFree(L.d_u[0]); cudaFree(L.d_u[1]);
   cudaFree(L.d_part); cudaFree(L.d_dt); cudaFree(L.d_out); cudaFree(L.d_hist); cudaFree(L.d_mhdw); cudaFree(L.d_refined);
-  cudaFree(L.d_f);
+  cudaFree(L.d_f); cudaFree(L.d_pfix);
   for (auto& r : L.regions) cudaFree(r.d_slots);
   for (auto& p : L.peers) { cudaFree(p.d_recv); cudaFree(p.d_emit); cudaFree(p.d_sbuf); cudaFree(p.d_rbuf); }
   L = Level();
@@ -599,6 +605,17 @@ cudaError_t dispatch_sweep_grav(int riemann, const SweepArgs& a, int nb, cudaStr
     case RGPU_RIEMANN_ACOUSTIC: return launch_sweep_dense_grav<ND, RIEMANN_ACOUSTIC, AMRV>(a, nb, st);
     case RGPU_RIEMANN_HLLC: return launch_sweep_dense_grav<ND, RIEMANN_HLLC, AMRV>(a, nb, st);
     default: return launch_sweep_dense_grav<ND, RIEMANN_HLL, AMRV>(a, nb, st);
+  }
+}
+// pressure_fix: the PFIX instantiations of the 3-D AMR variant; GRAV: with poisson
+template <bool GRAV>
+cudaError_t dispatch_sweep_pfix(int riemann, const SweepArgs& a, int nb, cudaStream_t st) {
+  switch (riemann) {
+    case RGPU_RIEMANN_LLF: return launch_sweep_dense_pfix<RIEMANN_LLF, GRAV>(a, nb, st);
+    case RGPU_RIEMANN_EXACT: return launch_sweep_dense_pfix<RIEMANN_EXACT, GRAV>(a, nb, st);
+    case RGPU_RIEMANN_ACOUSTIC: return launch_sweep_dense_pfix<RIEMANN_ACOUSTIC, GRAV>(a, nb, st);
+    case RGPU_RIEMANN_HLLC: return launch_sweep_dense_pfix<RIEMANN_HLLC, GRAV>(a, nb, st);
+    default: return launch_sweep_dense_pfix<RIEMANN_HLL, GRAV>(a, nb, st);
   }
 }
 inline int need_force(const Level& L) {
@@ -913,6 +930,11 @@ int amr_godunov_dense(AmrLevel& A, int ilevel, double dt, const double* dt_dev) 
   amr_gather_slots_kernel<<<nb, nthr, 0, G.stream>>>(G.d_uold, L.d_u[0], L.d_slot_igrid, L.nslot, G.ncoarse, G.ngridmax, G.ncell, G.p.nvar, T_());
   amr_gather_slots_kernel<<<nb, nthr, 0, G.stream>>>(G.d_unew, L.d_u[1], L.d_slot_igrid, L.nslot, G.ncoarse, G.ngridmax, G.ncell, G.p.nvar, T_());
   CUDA_OK(cudaGetLastError());
+  if (G.p.pressure_fix) {   // divu, enew (columns nvar, nvar+1 of unew: set_unew's values + the finer level's refluxes)
+    amr_gather_slots_kernel<<<nb, nthr, 0, G.stream>>>(d_divu(), L.d_pfix, L.d_slot_igrid, L.nslot, G.ncoarse, G.ngridmax, G.ncell, 2, T_());
+    CUDA_OK(cudaGetLastError());
+    A.launches++;
+  }
   if (G.p.poisson) {   // f of every oct of the box (the host may upload a new f every step); a patch's empty shell slots take the
                        // f of their father cell (gloc gather, godunov_fine.f90:637-647)
     amr_gather_slots_kernel<<<nb, nthr, 0, G.stream>>>(G.d_force, L.d_f, L.d_slot_igrid, L.nslot, G.ncoarse, G.ngridmax, G.ncell, G.p.ndim, T_());
@@ -941,8 +963,13 @@ int amr_godunov_dense(AmrLevel& A, int ilevel, double dt, const double* dt_dev) 
   a.dx_pow2 = (std::frexp(L.dx, &ex) == 0.5) ? 1 : 0;
   a.ntx = L.ntx; a.nty = L.nty; a.nwork = L.nwork; a.part = nullptr; a.refined = L.d_refined;
   cudaError_t e;
-  if (G.p.poisson) {   // predictor only: set_uold and courant_fine apply the gravity terms through their list kernels
-    a.force = L.d_f; a.gsrc = 0;
+  if (G.p.poisson) { a.force = L.d_f; a.gsrc = 0; }   // predictor only: set_uold and courant_fine apply the gravity terms
+                                                      // through their list kernels
+  if (G.p.pressure_fix) {   // tmp1 / tmp2 into divu / enew; set_uold's pdV source and energy switch run as list kernels
+    a.pfix = L.d_pfix;
+    e = G.p.poisson ? dispatch_sweep_pfix<true>(G.p.riemann, a, L.nblocks, G.stream)
+                    : dispatch_sweep_pfix<false>(G.p.riemann, a, L.nblocks, G.stream);
+  } else if (G.p.poisson) {
     e = dispatch_sweep_grav<3, true>(G.p.riemann, a, L.nblocks, G.stream);
   } else
   switch (G.p.riemann) {
@@ -956,6 +983,11 @@ int amr_godunov_dense(AmrLevel& A, int ilevel, double dt, const double* dt_dev) 
   amr_scatter_slots_kernel<<<nb, nthr, 0, G.stream>>>(G.d_unew, L.d_u[1], L.d_slot_igrid, L.nslot, G.ncoarse, G.ngridmax, G.ncell, G.p.nvar, T_(), L.g);
   CUDA_OK(cudaGetLastError());
   A.launches += 4;
+  if (G.p.pressure_fix) {
+    amr_scatter_slots_kernel<<<nb, nthr, 0, G.stream>>>(d_divu(), L.d_pfix, L.d_slot_igrid, L.nslot, G.ncoarse, G.ngridmax, G.ncell, 2, T_(), L.g);
+    CUDA_OK(cudaGetLastError());
+    A.launches++;
+  }
   if (A.patch && A.nsurf > 0) {   // fluxes through the outer faces of the surface octs, then the coarse reflux pass
     AmrSweepArgs s{};
     s.t = amr_tree();
@@ -964,7 +996,8 @@ int amr_godunov_dense(AmrLevel& A, int ilevel, double dt, const double* dt_dev) 
     s.P = G.phys; s.dt = dt; s.dt_dev = dt_dev; s.dx = A.dx; s.inv_dx = 1.0 / A.dx; s.dx_pow2 = a.dx_pow2;
     s.interpol_type = G.interpol_type; s.interpol_var = G.interpol_var; s.difmag = 0.0; s.nps = 0;
     s.flux_only = 1; s.rflux_index = A.d_surf_io;
-    s.force = G.p.poisson ? G.d_force : nullptr; s.pfix = 0; s.nvr = G.nvn;   // the refluxed faces carry the gravity predictor
+    // the refluxed faces carry the gravity predictor and, with pressure_fix, tmp1 / tmp2 behind the fluxes
+    s.force = G.p.poisson ? G.d_force : nullptr; s.pfix = G.p.pressure_fix ? 1 : 0; s.nvr = G.nvn;
     e = dispatch_amr_nd<3>(G.p.riemann, s, G.stream);
     if (e != cudaSuccess) return fail(RGPU_ECUDA, "patch surface flux launch: %s", cudaGetErrorString(e));
     A.launches++;
@@ -972,9 +1005,9 @@ int amr_godunov_dense(AmrLevel& A, int ilevel, double dt, const double* dt_dev) 
   if (A.nent > 0) {
     RefluxArgs r{};
     r.nent = A.nent; r.cell = A.d_rcell; r.start = A.d_rstart; r.src = A.d_rsrc; r.rflux = A.d_rflux; r.unew = G.d_unew;
-    r.ncell = G.ncell; r.nvar = G.p.nvar; r.nsides = 2 * G.p.ndim; r.nsf = 1 << (G.p.ndim - 1);
+    r.ncell = G.ncell; r.nvar = G.nvn; r.nsides = 2 * G.p.ndim; r.nsf = 1 << (G.p.ndim - 1);   // nvn: divu / enew reflux like variables
     r.oneontwotondim = 1.0 / (double)(1 << G.p.ndim);
-    const int n = A.nent * G.p.nvar;
+    const int n = A.nent * G.nvn;
     amr_reflux_kernel<<<(n + 127) / 128, 128, 0, G.stream>>>(r);
     CUDA_OK(cudaGetLastError());
     A.launches++;
@@ -1650,6 +1683,10 @@ static int alloc_dense_store(Level& L, int ncpu, int nboundary, const int* bound
     CUDA_OK(cudaMalloc(&L.d_f, sizeof(double) * nd * T_() * nslot));
     CUDA_OK(cudaMemset(L.d_f, 0, sizeof(double) * nd * T_() * nslot));
   }
+  if (G.p.pressure_fix) {
+    CUDA_OK(cudaMalloc(&L.d_pfix, sizeof(double) * 2 * T_() * nslot));
+    CUDA_OK(cudaMemset(L.d_pfix, 0, sizeof(double) * 2 * T_() * nslot));
+  }
   L.regions.resize(nboundary);
   for (int b = 0; b < nboundary; b++) {
     L.regions[b].type = boundary_type[b];
@@ -1796,8 +1833,9 @@ int rgpu_bind_level(int ilevel, int ngrid_active, const int* igrid_active, int n
     if (L.bound) free_level(L);
     const char* env = getenv("RGPU_AMR_DENSE");
     const char* envp = getenv("RGPU_AMR_PATCH");
+    // poisson: GRAV variant; pressure_fix: PFIX variant (both: GRAV+PFIX)
     const bool eligible = !(env && atoi(env) == 0) && G.p.ndim == 3 && !G.p.mhd && !(G.p.difmag > 0.0) && G.p.nvar == G.p.ndim + 2 &&
-                          ngrid_active > 0 && !G.p.pressure_fix;   // pressure_fix: oct-batch kernel only (poisson: GRAV variant)
+                          ngrid_active > 0;
     const bool base = eligible && A.nent == 0 && ncpu == 1;   // multi-rank AMR keeps the oct-batch kernel (tested path)
     // a refined level whose octs form a Cartesian box (nested / zoom refinement): dense kernel on the box + a prolongated
     // ghost shell; the octs at its surface go through the oct-batch kernel once more for the refluxed faces only
@@ -1846,7 +1884,7 @@ int rgpu_bind_level(int ilevel, int ngrid_active, const int* igrid_active, int n
   // poisson runs through the dense sweep's GRAV instantiation (rgpu_init admits it for nvar = ndim+2, difmag = 0 only)
   if (G.p.difmag > 0.0 || (!G.p.mhd && G.p.nvar != G.p.ndim + 2) || G.p.pressure_fix)
     return fail(RGPU_EUNSUPPORTED, "difmag>0 (cmpdivu/consup), passive scalars (nvar>ndim+2) and pressure_fix (also with poisson) are built in "
-                                   "the oct-batch kernel only: call rgpu_set_amr(1, interpol_type, 0) after rgpu_init (works for levelmin=levelmax "
+                                   "AMR mode only: call rgpu_set_amr(1, interpol_type, 0) after rgpu_init (works for levelmin=levelmax "
                                    "runs too)");
   Level& L = G.lev[ilevel];
   if (L.bound) free_level(L);

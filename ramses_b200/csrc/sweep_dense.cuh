@@ -75,6 +75,10 @@ struct SweepArgs {
   const double* force;
   int gsrc;                   // 1: set_uold's add_gravity_source_terms is fused into the update and the Courant scan of the
                               // new state uses sum|f| (rgpu_level_steps: f stays fixed over the steps of the call)
+  // pressure_fix (PFIX instantiation, AMR variant only): divu and enew in the level-store layout [2][2^ndim][nslot] (addressed
+  // like uout).  On entry they hold set_unew's values plus the finer level's refluxes; the sweep accumulates the face velocity
+  // tmp1 and the internal-energy flux tmp2 into them like two more variables (hydro/godunov_fine.f90:735-745,775-786)
+  double* pfix;
 };
 
 __device__ __forceinline__ int wrap_or_clamp(int c, int n, int wrap) {
@@ -177,7 +181,7 @@ __device__ __forceinline__ void cp_async8(double* smem_dst, const double* gsrc) 
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
 #endif
 
-template <int NDIM, int BX, int BY, bool GRAV = false>
+template <int NDIM, int BX, int BY, bool GRAV = false, bool PFIX = false>
 struct SweepSmem {
   static constexpr int NV = NDIM + 2;
   static constexpr int HY = (NDIM > 1) ? 1 : 0;
@@ -192,7 +196,9 @@ struct SweepSmem {
   static constexpr size_t exq = HY ? (size_t)NV * NT : 0;  // qm_y
   static constexpr size_t exf = HY ? (size_t)NV * NT : 0;  // Fy
   static constexpr size_t carry = HZ ? (size_t)3 * NV * NT : 0;
-  static constexpr size_t doubles = ring + stage + fstage + exq + exf + carry;
+  static constexpr size_t exft = PFIX ? (size_t)2 * NT : 0;    // tmp1, tmp2 of the y faces
+  static constexpr size_t carryt = PFIX ? (size_t)4 * NT : 0;  // tmp1, tmp2 of the previous z face, partial divu / enew update
+  static constexpr size_t doubles = ring + stage + fstage + exq + exf + carry + exft + carryt;
 };
 
 // LATE (experimental, not dispatched by the product yet; exercised by tests/host_numerics): the x/y part of the update of plane k
@@ -200,11 +206,15 @@ struct SweepSmem {
 // are complete by then -- so the plane loop has two CTA barriers instead of three.  Same arithmetic in the same order.
 // GRAV (poisson): the gravity predictor with f = a.force in ctoprim of every converted cell and, when a.gsrc is set, set_uold's
 // add_gravity_source_terms in the update plus the gravity term of the fused Courant scan.
-template <int NDIM, int RIEMANN, int SLOPE, int BX, int BY, bool AMRV = false, bool LATE = false, bool GRAV = false>
+// PFIX (pressure_fix, 3-D AMR variant): every face also yields tmp1 = half*(ql(ln)+qr(ln)) and tmp2 = the internal-energy flux of
+// the solver (hydro/umuscl.f90:844-850), scaled and masked like the fluxes; the update accumulates them into divu / enew
+// (a.pfix) in the same x, y, z order.  They travel like the fluxes: x by shuffle, y through shared memory, z in the carry.
+template <int NDIM, int RIEMANN, int SLOPE, int BX, int BY, bool AMRV = false, bool LATE = false, bool GRAV = false, bool PFIX = false>
 __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs a) {
   static_assert(!(LATE && AMRV), "the late-update variant exists for the plain dense sweep only");
   static_assert(!(LATE && GRAV), "the late-update variant exists for the plain dense sweep only");
-  using S = SweepSmem<NDIM, BX, BY, GRAV>;
+  static_assert(!PFIX || (AMRV && NDIM == 3), "pressure_fix exists for the 3-D AMR variant only");
+  using S = SweepSmem<NDIM, BX, BY, GRAV, PFIX>;
   constexpr int NV = S::NV, HY = S::HY, HZ = S::HZ, QX = S::QX, QY = S::QY, NQ = S::NQ, NT = S::NT;
   constexpr int TXO = BX - 2;                 // owned cells per tile in x
   constexpr int TYO = HY ? BY - 2 : 1;
@@ -222,6 +232,9 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
   double* exq = fstg + S::fstage;              // [NV][NT] qm_y
   double* exf = exq + S::exq;                  // [NV][NT] Fy
   double* carry = exf + S::exf;                // [3][NV][NT]: qm_z, Fz, partial update of the previous plane
+  double* exft = carry + S::carry;             // PFIX: [2][NT] tmp1, tmp2 of the y faces
+  double* carryt = exft + S::exft;             // PFIX: [4][NT] tmp1, tmp2 of the z face below, partial divu / enew update
+  constexpr int NPF = PFIX ? 2 : 1;            // tmp1, tmp2
   __shared__ double red[4][NT / 32];
   __shared__ unsigned char exm[AMRV ? NT : 1];   // AMRV: refined flag of every thread's cell (y exchange)
 
@@ -503,18 +516,31 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
       __syncthreads();
 
       double fx[NV], fy[NV], fz[NV], ucur[NV];
+      double tx[NPF], ty[NPF], tz[NPF], pcur[NPF];   // PFIX: tmp1, tmp2 of my -x, -y, -z faces; divu, enew of my cell
 #pragma unroll
       for (int n = 0; n < NV; n++) { fx[n] = 0.0; fy[n] = 0.0; fz[n] = 0.0; ucur[n] = 0.0; }
+#pragma unroll
+      for (int n = 0; n < NPF; n++) { tx[n] = 0.0; ty[n] = 0.0; tz[n] = 0.0; pcur[n] = 0.0; }
       if (own && plane_flux) {   // set_unew: unew = uold; issued early so the latency hides under the Riemann solves
         const long long off = cell_offset<NDIM>(g, cx, cy, HZ ? k : 0);
         if (AMRV) {              // unew already holds uold + the refluxes of the finer level (godunov_fine.f90:751-792 adds to it)
 #pragma unroll
           for (int n = 0; n < NV; n++) ucur[n] = a.uout[n * vstride + off];
+          if (PFIX) {
+#pragma unroll
+            for (int n = 0; n < NPF; n++) pcur[n] = a.pfix[n * vstride + off];
+          }
         } else {
 #pragma unroll
           for (int n = 0; n < NV; n++) ucur[n] = __ldg(a.uin + n * vstride + off);
         }
       }
+      // PFIX: tmp1 = half*(qleft(ln)+qright(ln)), tmp2 = fgdnv(nvar+1) (hydro/umuscl.f90:844-850), scaled like the fluxes (:111-112)
+      auto pfix_face = [&](const double* ql, const double* qr, double fe, double* t) {
+        t[0] = 0.5 * (ql[1] + qr[1]);
+        t[NPF - 1] = fe;
+        scale_fluxes<NPF>(t, dt, a.dx, a.inv_dx, a.dx_pow2);
+      };
       // ---- X faces: cmpflxm(...,2,3,4) hydro/umuscl.f90:97 ----
       if (need_fx && plane_flux) {
         double ql[NV], qr[NV], fg[NV];
@@ -528,14 +554,18 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
         qr[0] = qp[0]; qr[1] = qp[1]; qr[2] = qp[NDIM + 1];
         if (NDIM > 1) qr[3] = qp[2];
         if (NDIM > 2) qr[4] = qp[3];
-        riemann<NDIM, RIEMANN>(ql, qr, fg, P);
+        double fe = 0.0;
+        riemann<NDIM, RIEMANN>(ql, qr, fg, P, PFIX ? &fe : nullptr);
         fx[0] = fg[0]; fx[1] = fg[1]; fx[NDIM + 1] = fg[2];
         if (NDIM > 1) fx[2] = fg[3];
         if (NDIM > 2) fx[3] = fg[4];
         scale_fluxes<NV>(fx, dt, a.dx, a.inv_dx, a.dx_pow2);
+        if (PFIX) pfix_face(ql, qr, fe, tx);
         if (AMRV && (mlx | mc)) {   // reset flux along direction at refined interface :720-747
 #pragma unroll
           for (int n = 0; n < NV; n++) fx[n] = 0.0;
+#pragma unroll
+          for (int n = 0; n < NPF; n++) tx[n] = 0.0;
         }
       }
       // ---- Y faces: cmpflxm(...,3,2,4) hydro/umuscl.f90:120 ----
@@ -550,16 +580,24 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
         if (qp[0] < P.smallr) qp[0] = q[0];
         qr[0] = qp[0]; qr[1] = qp[2]; qr[2] = qp[NDIM + 1]; qr[3] = qp[1];
         if (NDIM > 2) qr[4] = qp[3];
-        riemann<NDIM, RIEMANN>(ql, qr, fg, P);
+        double fe = 0.0;
+        riemann<NDIM, RIEMANN>(ql, qr, fg, P, PFIX ? &fe : nullptr);
         fy[0] = fg[0]; fy[2] = fg[1]; fy[NDIM + 1] = fg[2]; fy[1] = fg[3];
         if (NDIM > 2) fy[3] = fg[4];
         scale_fluxes<NV>(fy, dt, a.dx, a.inv_dx, a.dx_pow2);
+        if (PFIX) pfix_face(ql, qr, fe, ty);
         if (AMRV && (exm[AMRV ? tid - BX : 0] | mc)) {
 #pragma unroll
           for (int n = 0; n < NV; n++) fy[n] = 0.0;
+#pragma unroll
+          for (int n = 0; n < NPF; n++) ty[n] = 0.0;
         }
 #pragma unroll
         for (int n = 0; n < NV; n++) exf[n * NT + tid] = fy[n];
+        if (PFIX) {
+#pragma unroll
+          for (int n = 0; n < NPF; n++) exft[n * NT + tid] = ty[n];
+        }
       }
       // ---- Z faces: cmpflxm(...,4,2,3) hydro/umuscl.f90:144; left state carried from the previous plane ----
       if (HZ && own && k >= z0) {
@@ -571,12 +609,16 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
         for (int n = 0; n < NV; n++) qp[n] = q[n] - 0.5 * dq[NDIM - 1][n] + t0[n];
         if (qp[0] < P.smallr) qp[0] = q[0];
         qr[0] = qp[0]; qr[1] = qp[3 % NV]; qr[2] = qp[NDIM + 1]; qr[3] = qp[1]; qr[4 % NV] = qp[2];
-        riemann<NDIM, RIEMANN>(ql, qr, fg, P);
+        double fe = 0.0;
+        riemann<NDIM, RIEMANN>(ql, qr, fg, P, PFIX ? &fe : nullptr);
         fz[0] = fg[0]; fz[3 % NV] = fg[1]; fz[NDIM + 1] = fg[2]; fz[1] = fg[3]; fz[2] = fg[4 % NV];
         scale_fluxes<NV>(fz, dt, a.dx, a.inv_dx, a.dx_pow2);
+        if (PFIX) pfix_face(ql, qr, fe, tz);
         if (AMRV && (mprev | mc)) {
 #pragma unroll
           for (int n = 0; n < NV; n++) fz[n] = 0.0;
+#pragma unroll
+          for (int n = 0; n < NPF; n++) tz[n] = 0.0;
         }
       }
       mprev = mc;
@@ -592,21 +634,35 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
       double fxr[NV];
 #pragma unroll
       for (int n = 0; n < NV; n++) fxr[n] = __shfl_down_sync(0xffffffffu, fx[n], 1);
+      double txr[NPF];
+      if (PFIX) {
+#pragma unroll
+        for (int n = 0; n < NPF; n++) txr[n] = __shfl_down_sync(0xffffffffu, tx[n], 1);
+      }
       if (!LATE) __syncthreads();
 
       // ---- conservative update (godfine1, hydro/godunov_fine.f90:751-792): x, then y, then z ----
+      // PFIX: divu, enew accumulate tmp1, tmp2 in the same order (:775-786)
       if (own) {
-        double unew_[NV];
+        double unew_[NV], pnew[NPF];
         bool have = false;
         if (HZ) {
           if (k > z0) {   // finish plane k-1 with the z fluxes
 #pragma unroll
             for (int n = 0; n < NV; n++) unew_[n] = carry[(2 * NV + n) * NT + tid] + (carry[(NV + n) * NT + tid] - fz[n]);
+            if (PFIX) {
+#pragma unroll
+              for (int n = 0; n < NPF; n++) pnew[n] = carryt[(2 + n) * NT + tid] + (carryt[n * NT + tid] - tz[n]);
+            }
             have = true;
           }
           if (k >= z0) {
 #pragma unroll
             for (int n = 0; n < NV; n++) carry[(NV + n) * NT + tid] = fz[n];
+            if (PFIX) {
+#pragma unroll
+              for (int n = 0; n < NPF; n++) carryt[n * NT + tid] = tz[n];
+            }
           }
         }
         if (plane_flux && LATE) {
@@ -627,6 +683,15 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
             if (HY) u = u + (fy[n] - exf[n * NT + tid + BX]);
             if (HZ) carry[(2 * NV + n) * NT + tid] = u; else unew_[n] = u;
           }
+          if (PFIX) {
+#pragma unroll
+            for (int n = 0; n < NPF; n++) {
+              double p = pcur[n];
+              p = p + (tx[n] - txr[n]);
+              p = p + (ty[n] - exft[n * NT + tid + BX]);
+              carryt[(2 + n) * NT + tid] = p;
+            }
+          }
           if (!HZ) have = true;
         }
         if (have) {
@@ -646,6 +711,10 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
           }
 #pragma unroll
           for (int n = 0; n < NV; n++) a.uout[n * vstride + off] = unew_[n];   // set_uold: uold = unew
+          if (PFIX) {
+#pragma unroll
+            for (int n = 0; n < NPF; n++) a.pfix[n * vstride + off] = pnew[n];
+          }
           // fused courant_fine of the new state (hydro/courant_fine.f90:96-123)
           double ei;
           const double dtc = cmpdt_cell<NDIM>(unew_, a.dx, P, ei, gsum);
@@ -758,6 +827,22 @@ cudaError_t launch_sweep_dense_grav(const SweepArgs& a, int nblocks, cudaStream_
   constexpr int BX = 32, BY = tile_by_default(NDIM, RIEMANN);
   constexpr size_t smem = sizeof(double) * SweepSmem<NDIM, BX, BY, true>::doubles;
   auto kern = sweep_dense_kernel<NDIM, RIEMANN, -1, BX, BY, AMRV, false, true>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    configured = true;
+  }
+  kern<<<nblocks, dim3(BX, BY, 1), smem, st>>>(a);
+  return cudaGetLastError();
+}
+// pressure_fix (PFIX): the 3-D AMR variant, one instantiation per solver without and with poisson (sweep_pfix_inst_3d_*.cu),
+// runtime slope switch and 12-row tiles
+template <int RIEMANN, bool GRAV>
+cudaError_t launch_sweep_dense_pfix(const SweepArgs& a, int nblocks, cudaStream_t st) {
+  constexpr int BX = 32, BY = tile_by_default(3, RIEMANN);
+  constexpr size_t smem = sizeof(double) * SweepSmem<3, BX, BY, GRAV, true>::doubles;
+  auto kern = sweep_dense_kernel<3, RIEMANN, -1, BX, BY, true, false, GRAV, true>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
