@@ -22,14 +22,15 @@ class MhdAmrRun(AmrRun):
     def __init__(self, levelmin, levelmax, bound_type, boxlen, nsubcycle, riemann="hlld", slope_type=1, gamma=1.4,
                  courant_factor=0.8, err_grad_d=-1.0, err_grad_u=-1.0, err_grad_p=-1.0, err_grad_A=-1.0, err_grad_B=-1.0,
                  err_grad_C=-1.0, err_grad_B2=-1.0, interpol_type=1, regions=(), tout=(), nexpand=1, ngridmax=2000, nvector=32,
-                 smallr=1e-10, smallc=1e-10):
+                 smallr=1e-10, smallc=1e-10, slope_mag_type=-1, coarse=(1, 1, 1)):
         super().__init__(1, levelmin, levelmax, bound_type, boxlen, nsubcycle, nexpand=nexpand, ngridmax=ngridmax,
                          riemann="llf", slope_type=slope_type, gamma=gamma, courant_factor=courant_factor,
                          err_grad_d=err_grad_d, err_grad_u=err_grad_u, err_grad_p=err_grad_p, interpol_type=interpol_type,
-                         interpol_var=0, regions=regions, tout=tout, nvector=nvector)
-        self.pm = orc.make_mhd_params(slope_type=slope_type, riemann=riemann, riemann2d="llf", gamma=gamma,
-                                      courant_factor=courant_factor, boxlen=boxlen, smallr=smallr, smallc=smallc)
+                         interpol_var=0, regions=regions, tout=tout, nvector=nvector, coarse=coarse)
+        self.pm = orc.make_mhd_params(slope_type=slope_type, slope_mag_type=slope_mag_type, riemann=riemann, riemann2d="llf",
+                                      gamma=gamma, courant_factor=courant_factor, boxlen=boxlen, smallr=smallr, smallc=smallc)
         self.p.smallr, self.p.smallc = smallr, smallc      # the driver's own floors (dtnew = boxlen / smallc, region fill)
+        self.interpol_type, self.interpol_mag_type = interpol_type, -1
         self.nvar = NVS                                   # stored variables (nvar+3 of the MHD build)
         self.uold = np.zeros(NVS * self.ncell)
         self.unew = np.zeros(NVS * self.ncell)
@@ -44,12 +45,19 @@ class MhdAmrRun(AmrRun):
         L.orc_mhd1_courant_fine.argtypes = [pp, mp, C.c_int, C.c_double, dp]
         L.orc_mhd1_make_boundary_hydro.argtypes = [pp, mp, C.c_int, dp]
         L.orc_mhd1_upload_fine.argtypes = [pp, mp, C.c_int, dp]
+        L.orc_mhd_set_interpol.argtypes = [C.c_int, C.c_int]
+
+    def use_interpol(self):
+        """the oracle's prolongation limiters are process globals: make them this run's before every routine that reads them
+        (several runs may live side by side in one process)"""
+        self.L.orc_mhd_set_interpol(self.interpol_type, self.interpol_mag_type)
 
     # ---- floating-point routines -------------------------------------------------------------------------------------
     def c_set_unew(self, l):
         self.L.orc_mhdn_set_unew(self.mp, l, orc.dptr(self.uold), orc.dptr(self.unew))
 
     def c_godunov_fine(self, l):
+        self.use_interpol()
         self.L.orc_mhd1_godunov_fine(C.byref(self.pm), self.mp, l, self.levelmin, self.nvector, self.dtnew[l], orc.dptr(self.uold),
                                      orc.dptr(self.unew))
 
@@ -58,6 +66,7 @@ class MhdAmrRun(AmrRun):
 
     def c_interpol_cell(self, c, lnew):
         u2 = np.zeros(2 * NVS)
+        self.use_interpol()
         self.L.orc_mhd1_interpol_cell(self.mp, c, lnew, orc.dptr(self.uold), orc.dptr(u2))
         return u2
 
@@ -235,13 +244,14 @@ class MhdAmrRun2D(FastAmrRun):
     def __init__(self, levelmin, levelmax, boxlen, nsubcycle, riemann="hlld", riemann2d="hlld", slope_type=2, gamma=1.4,
                  courant_factor=0.8, err_grad_d=-1.0, err_grad_u=-1.0, err_grad_p=-1.0, err_grad_A=-1.0, err_grad_B=-1.0,
                  err_grad_C=-1.0, err_grad_B2=-1.0, interpol_type=2, tout=(), nexpand=1, ngridmax=100000, nvector=32,
-                 ic="orszag_tang", nthreads=None, smallr=1e-10, smallc=1e-10):
+                 ic="orszag_tang", nthreads=None, smallr=1e-10, smallc=1e-10, slope_mag_type=-1, interpol_mag_type=-1, coarse=(1, 1, 1)):
         super().__init__(self.NDIM, levelmin, levelmax, (0, 0, 0, 0, 0, 0), boxlen, nsubcycle, nexpand=nexpand, ngridmax=ngridmax,
                          riemann="llf", slope_type=slope_type, gamma=gamma, courant_factor=courant_factor,
                          err_grad_d=err_grad_d, err_grad_u=err_grad_u, err_grad_p=err_grad_p, interpol_type=interpol_type,
-                         interpol_var=0, regions=(), tout=tout, nvector=nvector, nthreads=nthreads)
-        self.pm = orc.make_mhd_params(slope_type=slope_type, riemann=riemann, riemann2d=riemann2d, gamma=gamma,
-                                      courant_factor=courant_factor, boxlen=boxlen, smallr=smallr, smallc=smallc)
+                         interpol_var=0, regions=(), tout=tout, nvector=nvector, nthreads=nthreads, coarse=coarse)
+        self.pm = orc.make_mhd_params(slope_type=slope_type, slope_mag_type=slope_mag_type, riemann=riemann, riemann2d=riemann2d,
+                                      gamma=gamma, courant_factor=courant_factor, boxlen=boxlen, smallr=smallr, smallc=smallc)
+        self.interpol_type, self.interpol_mag_type = interpol_type, interpol_mag_type
         self.p.smallr, self.p.smallc = smallr, smallc
         self.nvar = NVS
         self.uold = np.zeros(NVS * self.ncell)
@@ -251,7 +261,7 @@ class MhdAmrRun2D(FastAmrRun):
         self.flo7 = np.full(7, 1e-10)
         L, mp, pp, dp, ip = self.L, C.POINTER(orc.MeshS), C.POINTER(orc.MhdParams), C.POINTER(C.c_double), C.POINTER(C.c_int)
         L.orc_mhd_set_interpol.argtypes = [C.c_int, C.c_int]
-        L.orc_mhd_set_interpol(interpol_type, -1)
+        L.orc_mhd_set_interpol(interpol_type, interpol_mag_type)
         import os
         L.orc_mhd_set_threads.argtypes = [C.c_int]      # flux phase of a batch only; results do not depend on it
         L.orc_mhd_set_threads(int(nthreads) if nthreads else min(8, os.cpu_count() or 1))
@@ -274,7 +284,12 @@ class MhdAmrRun2D(FastAmrRun):
     def c_set_unew(self, l):
         self.L.orc_mhdn_set_unew(self.mp, l, orc.dptr(self.uold), orc.dptr(self.unew))
 
+    def use_interpol(self):
+        """as MhdAmrRun.use_interpol"""
+        self.L.orc_mhd_set_interpol(self.interpol_type, self.interpol_mag_type)
+
     def c_godunov_fine(self, l):
+        self.use_interpol()
         self._godunov(C.byref(self.pm), self.mp, l, self.levelmin, self.nvector, self.dtnew[l], orc.dptr(self.uold),
                                      orc.dptr(self.unew))
 
@@ -283,6 +298,7 @@ class MhdAmrRun2D(FastAmrRun):
 
     def c_interpol_cell(self, c, lnew):
         u2 = np.zeros(self.T * NVS)
+        self.use_interpol()
         self._interpol(self.mp, c, lnew, orc.dptr(self.uold), orc.dptr(u2))
         return u2
 

@@ -154,7 +154,7 @@ def plan_level(amr, ilevel):
 class HydroGPU:
     """The patched routines of hydro/godunov_fine.f90 & friends, running on the GPU through the C-ABI."""
 
-    def __init__(self, amr: AmrCommons, device=-1, amr_mode=False, interpol_type=1, interpol_var=0):
+    def __init__(self, amr: AmrCommons, device=-1, amr_mode=False, interpol_type=1, interpol_var=0, interpol_mag_type=-1):
         self.a = amr
         self.L = _lib.load()
         p = make_params(amr)
@@ -162,8 +162,13 @@ class HydroGPU:
         _lib.check(self.L.rgpu_init(C.byref(p), amr.myid, amr.ncpu, device))
         if amr_mode:      # levelmin < nlevelmax: oct-list kernels on mirrored arrays
             _lib.check(self.L.rgpu_set_amr(1, interpol_type, interpol_var))
+            self.set_interpol_mag(interpol_mag_type)
         self._keep = []
         self.bind_tree()
+
+    def set_interpol_mag(self, interpol_mag_type):
+        """interpol_mag_type of the MHD build (face-field prolongation limiter; -1 = interpol_type), rgpu_set_interpol_mag"""
+        _lib.check(self.L.rgpu_set_interpol_mag(int(interpol_mag_type)))
 
     # -- bookkeeping the Fortran shim performs after build_comm / refine ------------------------------
     def bind_tree(self):

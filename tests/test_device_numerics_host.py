@@ -937,9 +937,10 @@ MHD_R2D = {"llf": 0, "roe": 1, "upwind": 2, "hll": 3, "hlla": 4, "hlld": 5}
 
 
 def _mhd_amr_compare_levels(orc, dev, r, ndim, riemann, riemann2d, slope_type, interpol_type, godunov, upload, courant, boundary=None,
-                            interpol_mag_type=-1):
+                            interpol_mag_type=-1, slope_mag_type=None):
     """every populated level of the run `r`: godunov_fine (own cells AND the refluxed coarse cells: the whole unew array),
-    upload_fine, the leaf-cell Courant step and (1-D) make_boundary_hydro of the device code == the oracle's, bit for bit"""
+    upload_fine, the leaf-cell Courant step and (1-D) make_boundary_hydro of the device code == the oracle's, bit for bit.
+    slope_mag_type: the face-field limiter handed to the device code (None: slope_type; r.pm carries the oracle's)"""
     m = r.m
     T, nc = 1 << ndim, r.ncell
     son = np.ascontiguousarray(r.son[1:], dtype=np.int32)
@@ -964,7 +965,7 @@ def _mhd_amr_compare_levels(orc, dev, r, ndim, riemann, riemann2d, slope_type, i
         before = unew_o.copy()
         godunov(C.byref(r.pm), r.mp, l, r.levelmin, r.nvector, dt, orc.dptr(r.uold), orc.dptr(unew_o))
         dev.devnum_mhd_amr_godunov(*tree[:9], orc.iptr(act), len(act), l, orc.dptr(r.uold), orc.dptr(unew_k), dt, dx, interpol_type, interpol_mag_type,
-                                   MHD_R1D[riemann], MHD_R2D[riemann2d], slope_type, slope_type, r.pm.gamma, r.pm.smallr, r.pm.smallc, r.nvector)
+                                   MHD_R1D[riemann], MHD_R2D[riemann2d], slope_type, slope_type if slope_mag_type is None else slope_mag_type, r.pm.gamma, r.pm.smallr, r.pm.smallc, r.nvector)
         assert np.isfinite(unew_k).all()
         assert np.array_equal(unew_k, unew_o), (l, np.abs(unew_k - unew_o).max())
         moved = max(moved, float(np.abs(unew_o - before).max()))

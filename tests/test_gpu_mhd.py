@@ -150,9 +150,11 @@ def test_mhd_rejects_unsupported():
     with pytest.raises(ValueError):
         HydroGPU(a)
     a = c.amr_commons()
-    a.slope_type = 7                               # the AMR-mode MHD kernels cover slope types 0, 1, 2
-    with pytest.raises(_l.RgpuError):
-        HydroGPU(a, amr_mode=True)
+    a.slope_type, a.slope_mag_type = 7, 1          # the AMR-mode MHD kernels cover slope types 0, 1, 2
+    HydroGPU(a).finalize()                         # rgpu_init accepts the pair (the dense sweep has slope type 7) ...
+    with pytest.raises(_l.RgpuError) as e:
+        HydroGPU(a, amr_mode=True)                 # ... rgpu_set_amr refuses it
+    assert e.value.code == -3 and "MHD AMR mode: slope_type=7" in str(e.value)   # RGPU_EUNSUPPORTED
     a = c.amr_commons()
     with pytest.raises(_l.RgpuError):
         HydroGPU(a, amr_mode=True, interpol_var=1)  # interpol_var = 0 only in the MHD build
@@ -240,7 +242,8 @@ def _mhd_commons_from_run(r, ndim, riemann, riemann2d, slope_type):
     a.gamma, a.courant_factor = r.pm.gamma, r.pm.courant_factor
     a.smallr, a.smallc = r.pm.smallr, r.pm.smallc
     a.slope_theta = r.pm.slope_theta
-    a.slope_type, a.slope_mag_type, a.riemann, a.riemann2d, a.nvector = slope_type, -1, riemann, riemann2d, r.nvector
+    smt = -1 if r.pm.slope_mag_type == slope_type else r.pm.slope_mag_type       # the oracle's face-field limiter
+    a.slope_type, a.slope_mag_type, a.riemann, a.riemann2d, a.nvector = slope_type, smt, riemann, riemann2d, r.nvector
     return a
 
 
