@@ -51,8 +51,10 @@ typedef struct rgpu_params {
   int scheme;          /* RGPU_SCHEME_MUSCL only                              */
   int riemann;         /* RGPU_RIEMANN_*                                       */
   int pressure_fix;    /* amr_parameters.f90:197.  1: divu / enew ride along the sweep (godfine1 :737-903), add_pdv_source_terms and
-                        * the energy switch of set_uold (:203-227, with beta_fix below).  Oct-batch kernel only (rgpu_set_amr),
-                        * nvar = ndim+2, difmag = 0; divu and enew live on the device (rgpu_download_pressure_fix)            */
+                        * the energy switch of set_uold (:203-227, with beta_fix below).  nvar = ndim+2, difmag = 0; oct-batch
+                        * kernel and the dense sweep (levelmin=levelmax levels, AMR base box and patches); outside AMR mode not
+                        * together with poisson.  divu and enew live on the device (rgpu_download_pressure_fix); rgpu_level_steps
+                        * takes dt from a Courant scan of the state after the energy switch                                   */
   double gamma, smallr, smallc, slope_theta, difmag, courant_factor;
                        /* difmag>0 (cmpdivu/consup, hydro/uplmde.f90:702,769): oct-batch kernel only, i.e. after rgpu_set_amr(1,..) */
   double boxlen;
@@ -73,7 +75,7 @@ typedef struct rgpu_params {
                         * (rgpu_upload_force; the Poisson solver is out of scope): gravity predictor of ctoprim (umuscl.f90:932-938),
                         * gloc gather of godfine1 (:637-647), add_gravity_source_terms in set_uold (:237-289), gravity term of cmpdt
                         * (godunov_utils.f90:99-111).  nvar = ndim+2, difmag = 0; oct-batch kernel and the dense sweep (levelmin=
-                        * levelmax levels, AMR base box and patches); with pressure_fix AMR mode only                              */
+                        * levelmax levels, AMR base box and patches); together with pressure_fix AMR mode only                     */
   double beta_fix;     /* amr_parameters.f90:167 (pressure_fix truncation-error factor)                                          */
 } rgpu_params;
 /* `riemann` / `riemann2d` of the MHD build: iriemann, iriemann2d (hydro/read_hydro_params.f90:190-220) */

@@ -683,14 +683,7 @@ __global__ void amr_pfix_init_kernel(const double* __restrict__ uold, double* __
   if (i >= n * T) return;
   const int o = i % n, ind = i / n;
   const size_t c = (size_t)ncoarse + (size_t)ind * ngridmax + igrid[o] - 1;
-  const double d = fmx(uold[c], smallr);
-  double u = 0, v = 0, w = 0;
-  if (ndim > 0) u = uold[(size_t)1 * ncell + c] / d;
-  if (ndim > 1) v = uold[(size_t)2 * ncell + c] / d;
-  if (ndim > 2) w = uold[(size_t)3 * ncell + c] / d;
-  const double e_kin = 0.5 * d * (u * u + v * v + w * w);
-  divu[c] = 0.0;
-  enew[c] = uold[(size_t)(ndim + 1) * ncell + c] - e_kin;
+  pfix_init_cell(uold + c, (size_t)ncell, divu + c, enew + c, ndim, smallr);
 }
 // add_gravity_source_terms (hydro/godunov_fine.f90:237-289)
 __global__ void amr_gravity_src_kernel(const double* __restrict__ uold, double* __restrict__ unew, const double* __restrict__ force,
@@ -736,18 +729,10 @@ __global__ void amr_pdv_kernel(const AmrTree t, const double* __restrict__ uold,
     else { const int g1 = t.son[cl_nb]; c1 = g1 > 0 ? amr_cell(t, other, g1) : cl_nb; dx_g = g1 > 0 ? dx_loc : dx_loc * 1.5; }
     if (b == 0) { c2 = amr_cell(t, other, ig); dx_d = dx_loc; }
     else { const int g2 = t.son[cr_nb]; c2 = g2 > 0 ? amr_cell(t, other, g2) : cr_nb; dx_d = g2 > 0 ? dx_loc : dx_loc * 1.5; }
-    const double velg = UO(c1, d + 1) / fmx(UO(c1, 0), smallr);
-    const double veld = UO(c2, d + 1) / fmx(UO(c2, 0), smallr);
-    divu_loc = divu_loc + (veld - velg) / (dx_g + dx_d);
+    divu_loc = pdv_face_term(divu_loc, UO, c1, c2, d, dx_g, dx_d, smallr);
   }
   const int ic = amr_cell(t, ind, ig);
-  const double dd = fmx(UO(ic, 0), smallr);
-  double u = 0, v = 0, w = 0;
-  if (ndim > 0) u = UO(ic, 1) / dd;
-  if (ndim > 1) v = UO(ic, 2) / dd;
-  if (ndim > 2) w = UO(ic, 3) / dd;
-  const double eold = UO(ic, ndim + 1) - 0.5 * dd * (u * u + v * v + w * w);
-  enew[ic - 1] = enew[ic - 1] - (gamma - 1.0) * eold * divu_loc * dtl;
+  enew[ic - 1] = pdv_cell(enew[ic - 1], divu_loc, UO, ic, ndim, gamma, smallr, dtl);
 }
 // set_uold, pressure_fix part (hydro/godunov_fine.f90:203-227), after uold <- unew: total energy = kinetic + enew where the
 // conservative internal energy is below the truncation error beta_fix*d*(|div u| dx)^2  (hexp = 0: no cosmology)
@@ -759,19 +744,7 @@ __global__ void amr_pfix_switch_kernel(double* __restrict__ uold, const double* 
   const int o = i % n, ind = i / n;
   const size_t c = (size_t)ncoarse + (size_t)ind * ngridmax + igrid[o] - 1;
   const double dtl = dt_dev ? *dt_dev : dt;
-  const double d = fmx(uold[c], smallr);
-  double u = 0, v = 0, w = 0;
-  if (ndim > 0) u = uold[(size_t)1 * ncell + c] / d;
-  if (ndim > 1) v = uold[(size_t)2 * ncell + c] / d;
-  if (ndim > 2) w = uold[(size_t)3 * ncell + c] / d;
-  const double e_kin = 0.5 * d * (u * u + v * v + w * w);
-  const double e_cons = uold[(size_t)(ndim + 1) * ncell + c] - e_kin;
-  const double e_prim = enew[c];
-  const double div = fabs(divu[c]) * dx / dtl;          // divu = -div.u*dt
-  const double hexp = 0.0;
-  const double mx = fmx(div, 3.0 * hexp * dx);
-  const double e_trunc = beta_fix * d * (mx * mx);
-  if (e_cons < e_trunc) uold[(size_t)(ndim + 1) * ncell + c] = e_prim + e_kin;
+  pfix_switch_cell(uold + c, (size_t)ncell, divu + c, enew + c, ndim, smallr, beta_fix, dx, dtl);
 }
 // ghost-oct exchange buffers on the mirrored arrays: all variables and all cells of the listed octs in one message
 // (make_virtual_fine_dp / make_virtual_reverse_dp, amr/virtual_boundaries.f90:373,693)

@@ -63,6 +63,12 @@ DECL(3, 0, true) DECL(3, 1, true) DECL(3, 2, true) DECL(3, 3, true) DECL(3, 4, t
 DECL(0, false) DECL(1, false) DECL(2, false) DECL(3, false) DECL(4, false)
 DECL(0, true) DECL(1, true) DECL(2, true) DECL(3, true) DECL(4, true)
 #undef DECL
+// pressure_fix outside AMR mode: the plain PFIX instantiations (sweep_pfix_inst_12d.cu, sweep_pfix_inst_plain3d_*.cu)
+#define DECL(ND, R) extern template cudaError_t launch_sweep_dense_pfix_plain<ND, R>(const SweepArgs&, int, cudaStream_t);
+DECL(1, 0) DECL(1, 1) DECL(1, 2) DECL(1, 3) DECL(1, 4)
+DECL(2, 0) DECL(2, 1) DECL(2, 2) DECL(2, 3) DECL(2, 4)
+DECL(3, 0) DECL(3, 1) DECL(3, 2) DECL(3, 3) DECL(3, 4)
+#undef DECL
 }  // namespace rgpu
 
 using namespace rgpu;
@@ -146,7 +152,8 @@ struct Level {
   double* d_mhdw = nullptr;          // MHD work arrays [MW_NCOMP][ncell_box]
   unsigned char* d_refined = nullptr;  // AMR mode: son(cell)>0 per box cell [2^ndim][nslot]
   double* d_f = nullptr;             // poisson: the acceleration f [ndim][2^ndim][nslot] (rgpu_upload_force; AMR mode: gathered per call)
-  double* d_pfix = nullptr;          // pressure_fix, AMR mode: divu and enew [2][2^ndim][nslot] (gathered from / scattered to d_unew per call)
+  double* d_pfix = nullptr;          // pressure_fix: divu and enew [2][2^ndim][nslot] (AMR mode: gathered from / scattered to d_unew per call)
+  bool pfix_ready = false;           // pressure_fix, levelmin=levelmax: set_unew has initialised divu / enew for the next sweep
   bool f_valid = false;              // poisson, levelmin=levelmax: f uploaded since the bind
   double dt_last = 0.0;              // dt of the last godunov_fine (rgpu_set_uold's gravity source term needs it)
   int mhd_nb = 0;                    // CTAs of the MHD update kernel
@@ -618,6 +625,17 @@ cudaError_t dispatch_sweep_pfix(int riemann, const SweepArgs& a, int nb, cudaStr
     default: return launch_sweep_dense_pfix<RIEMANN_HLL, GRAV>(a, nb, st);
   }
 }
+// pressure_fix outside AMR mode: the plain PFIX instantiations (runtime slope switch, default tile height)
+template <int ND>
+cudaError_t dispatch_sweep_pfix_plain(int riemann, const SweepArgs& a, int nb, cudaStream_t st) {
+  switch (riemann) {
+    case RGPU_RIEMANN_LLF: return launch_sweep_dense_pfix_plain<ND, RIEMANN_LLF>(a, nb, st);
+    case RGPU_RIEMANN_EXACT: return launch_sweep_dense_pfix_plain<ND, RIEMANN_EXACT>(a, nb, st);
+    case RGPU_RIEMANN_ACOUSTIC: return launch_sweep_dense_pfix_plain<ND, RIEMANN_ACOUSTIC>(a, nb, st);
+    case RGPU_RIEMANN_HLLC: return launch_sweep_dense_pfix_plain<ND, RIEMANN_HLLC>(a, nb, st);
+    default: return launch_sweep_dense_pfix_plain<ND, RIEMANN_HLL>(a, nb, st);
+  }
+}
 inline int need_force(const Level& L) {
   if (G.p.poisson && !L.f_valid) return fail(RGPU_EINVAL, "poisson: no rgpu_upload_force since the level was bound (the sweep and the Courant "
                                                          "scan need the acceleration f)");
@@ -678,9 +696,18 @@ int launch_sweep(Level& L, int zlo = -1, int zhi = -1, int part = 0, bool gsrc =
     nblocks = (int)std::min<long long>(L.nblocks, a.nwork);
     a.part = nullptr;
   }
+  if (G.p.pressure_fix) {   // divu / enew accumulate into the PFIX store; the Courant scan runs after set_uold's energy switch
+    a.pfix = L.d_pfix;
+    a.part = nullptr;
+  }
   if (G.timing) cudaEventRecord(G.ev0, G.stream);
   cudaError_t e;
-  if (G.p.poisson) {   // round-1 kernel with gravity (3-D: variant 0, FAST ignored; rgpu_bind_level)
+  if (G.p.pressure_fix) {   // round-1 kernel with pressure_fix (3-D: variant 0, FAST ignored; rgpu_bind_level)
+    if (G.p.ndim == 1) e = dispatch_sweep_pfix_plain<1>(G.p.riemann, a, nblocks, G.stream);
+    else if (G.p.ndim == 2) e = dispatch_sweep_pfix_plain<2>(G.p.riemann, a, nblocks, G.stream);
+    else e = dispatch_sweep_pfix_plain<3>(G.p.riemann, a, nblocks, G.stream);
+  }
+  else if (G.p.poisson) {   // round-1 kernel with gravity (3-D: variant 0, FAST ignored; rgpu_bind_level)
     if (G.p.ndim == 1) e = dispatch_sweep_grav<1, false>(G.p.riemann, a, nblocks, G.stream);
     else if (G.p.ndim == 2) e = dispatch_sweep_grav<2, false>(G.p.riemann, a, nblocks, G.stream);
     else e = dispatch_sweep_grav<3, false>(G.p.riemann, a, nblocks, G.stream);
@@ -757,6 +784,31 @@ int launch_courant(Level& L, double dt_cap, double* hist_slot) {
   CUDA_OK(cudaGetLastError());
   L.launches++;
   return launch_reduce(L, nb, dt_cap, hist_slot);
+}
+
+// pressure_fix passes on the owned cells of a dense level (sweep_dense.cuh).  dt_dev != NULL: the time step of rgpu_level_steps
+// (device resident), otherwise dt.  PFIX_INIT: set_unew's divu = 0, enew = e_int of uold; PFIX_PDV: add_pdv_source_terms from
+// uold, whose ghost and boundary shells must be current; PFIX_SWITCH: set_uold's energy switch on the new state (after the swap)
+enum PfixPass { PFIX_INIT, PFIX_PDV, PFIX_SWITCH };
+int launch_pfix_pass(Level& L, PfixPass k, double dt, const double* dt_dev) {
+  long long n = L.g.ox1 - L.g.ox0;
+  if (G.p.ndim > 1) n *= L.g.oy1 - L.g.oy0;
+  if (G.p.ndim > 2) n *= L.g.oz1 - L.g.oz0;
+  const unsigned nb = (unsigned)((n + 127) / 128);
+  const double* uo = L.d_u[L.cur];
+#define PFIX_LAUNCH(ND)                                                                                                          \
+  do {                                                                                                                           \
+    if (k == PFIX_INIT) dense_pfix_init_kernel<ND><<<nb, 128, 0, G.stream>>>(uo, L.d_pfix, L.g, G.p.smallr);                    \
+    else if (k == PFIX_PDV) dense_pdv_kernel<ND><<<nb, 128, 0, G.stream>>>(uo, L.d_pfix, L.g, G.p.gamma, G.p.smallr, L.dx, dt, dt_dev); \
+    else dense_pfix_switch_kernel<ND><<<nb, 128, 0, G.stream>>>(L.d_u[L.cur], L.d_pfix, L.g, G.p.smallr, G.p.beta_fix, L.dx, dt, dt_dev); \
+  } while (0)
+  if (G.p.ndim == 1) PFIX_LAUNCH(1);
+  else if (G.p.ndim == 2) PFIX_LAUNCH(2);
+  else PFIX_LAUNCH(3);
+#undef PFIX_LAUNCH
+  CUDA_OK(cudaGetLastError());
+  L.launches++;
+  return RGPU_OK;
 }
 
 int launch_boundaries(Level& L, double* u) {
@@ -1697,6 +1749,8 @@ static int alloc_dense_store(Level& L, int ncpu, int nboundary, const int* bound
     }
   }
   // ---- peers (ghost exchange lists) ----------------------------------------------------------
+  // The exchange carries the state only.  pressure_fix's divu / enew need no ghost exchange and no reverse accumulation on a
+  // full level: the pdV pass reads the neighbours' uold, and only a coarse-fine face (AMR mode) writes a neighbour's divu / enew.
   if (ncpu > 1) {
     L.peers.resize(ncpu);
     for (int c = 0; c < ncpu; c++) {
@@ -1747,11 +1801,12 @@ static int alloc_dense_store(Level& L, int ncpu, int nboundary, const int* bound
   // ---- tile decomposition of the owned range ----------------------------------------------------
   const int bx = 32;
   int by = tile_by_default(nd, G.p.riemann);
-  // poisson: the GRAV instantiations exist for the default tile height of the round-1 kernel only (variant 0, FAST ignored)
-  if (nd == 3 && !G.p.poisson) { const char* e = getenv("RGPU_BY3"); if (e) { const int v = atoi(e); if (v == 8 || v == 12 || v == 16) by = v; } }
+  // poisson, pressure_fix: the GRAV / PFIX instantiations exist for the default tile height of the round-1 kernel only (variant 0,
+  // FAST ignored)
+  if (nd == 3 && !G.p.poisson && !G.p.pressure_fix) { const char* e = getenv("RGPU_BY3"); if (e) { const int v = atoi(e); if (v == 8 || v == 12 || v == 16) by = v; } }
   int minb = 1;
   L.variant = 0;
-  if (nd == 3 && !G.p.mhd && !G.amr && !G.p.poisson) {   // plain dense 3-D sweep: round-2 kernel; RGPU_SWEEP=old|<variant> for tuning runs
+  if (nd == 3 && !G.p.mhd && !G.amr && !G.p.poisson && !G.p.pressure_fix) {   // plain dense 3-D sweep: round-2 kernel; RGPU_SWEEP=old|<variant> for tuning runs
     // the two-barrier loop (sweep3_kernel, three scalar branch-free solves); profiles/tune_sweep.py times the variants
     L.variant = SWEEP3_DEFAULT_VARIANT;
     const char* e = getenv("RGPU_SWEEP");
@@ -1881,11 +1936,12 @@ int rgpu_bind_level(int ilevel, int ngrid_active, const int* igrid_active, int n
   }
   if (G.p.mhd && G.p.ndim != 3)
     return fail(RGPU_EUNSUPPORTED, "MHD build, NDIM=%d: built in AMR mode only -- call rgpu_set_amr(1, interpol_type, 0) after rgpu_init", G.p.ndim);
-  // poisson runs through the dense sweep's GRAV instantiation (rgpu_init admits it for nvar = ndim+2, difmag = 0 only)
-  if (G.p.difmag > 0.0 || (!G.p.mhd && G.p.nvar != G.p.ndim + 2) || G.p.pressure_fix)
-    return fail(RGPU_EUNSUPPORTED, "difmag>0 (cmpdivu/consup), passive scalars (nvar>ndim+2) and pressure_fix (also with poisson) are built in "
-                                   "AMR mode only: call rgpu_set_amr(1, interpol_type, 0) after rgpu_init (works for levelmin=levelmax "
-                                   "runs too)");
+  // poisson and pressure_fix run through the dense sweep's GRAV / PFIX instantiations (rgpu_init admits them for nvar = ndim+2,
+  // difmag = 0 only); both together have no plain form
+  if (G.p.difmag > 0.0 || (!G.p.mhd && G.p.nvar != G.p.ndim + 2) || (G.p.pressure_fix && G.p.poisson))
+    return fail(RGPU_EUNSUPPORTED, "difmag>0 (cmpdivu/consup), passive scalars (nvar>ndim+2) and pressure_fix together with poisson are "
+                                   "built in AMR mode only: call rgpu_set_amr(1, interpol_type, 0) after rgpu_init (works for "
+                                   "levelmin=levelmax runs too)");
   Level& L = G.lev[ilevel];
   if (L.bound) free_level(L);
   {
@@ -1894,6 +1950,28 @@ int rgpu_bind_level(int ilevel, int ngrid_active, const int* igrid_active, int n
     if (rc) return rc;
   }
   if (!L.dense) return RGPU_OK;   // bound, but only the AMR path could run it
+  if (G.p.pressure_fix) {
+    // add_pdv_source_terms reads the face neighbours of every owned cell.  plan_level admits a shell with holes (it only bounds
+    // the shell's extent); where a face-neighbour oct is missing the reference would read the father cell 1.5 dx away, which a
+    // dense level does not hold: refuse such a level
+    const DenseGeom& g = L.g;
+    const int nd = G.p.ndim, wrap[3] = {g.wrapx, g.wrapy, g.wrapz};
+    const int o0[3] = {g.ox0 / 2, g.oy0 / 2, g.oz0 / 2}, o1[3] = {g.ox1 / 2, nd > 1 ? g.oy1 / 2 : 1, nd > 2 ? g.oz1 / 2 : 1};
+    const long long str[3] = {1, g.nox, (long long)g.nox * g.noy};
+    for (int oz = o0[2]; oz < o1[2]; oz++)
+      for (int oy = o0[1]; oy < o1[1]; oy++)
+        for (int ox = o0[0]; ox < o1[0]; ox++) {
+          const long long s0 = ox + str[1] * oy + str[2] * oz;
+          for (int d = 0; d < nd; d++)
+            for (int side = -1; side <= 1; side += 2)
+              if (!wrap[d] && L.slot_igrid[s0 + side * str[d]] <= 0) {
+                L = Level();
+                return fail(RGPU_EUNSUPPORTED, "pressure_fix: an active oct of level %d has no neighbour oct across its %s face along "
+                                               "dimension %d (outside AMR mode every face neighbour must be bound)", ilevel,
+                            side < 0 ? "lower" : "upper", d + 1);
+              }
+        }
+  }
   return alloc_dense_store(L, ncpu, nboundary, boundary_type);
 }
 
@@ -2081,6 +2159,7 @@ int rgpu_upload_state(int ilevel, const double* uold) {
   if (!uold) return fail(RGPU_EINVAL, "null uold");
   rc = upload_into(*L, uold, L->d_u[L->cur]); if (rc) return rc;
   L->unew_valid = false;
+  L->pfix_ready = false;
   return RGPU_OK;
 }
 int rgpu_download_state(int ilevel, double* uold) {
@@ -2108,6 +2187,10 @@ int rgpu_set_unew(int ilevel) {
       CUDA_OK(cudaGetLastError());
       L->launches++;
     }
+  if (G.p.pressure_fix) {   // divu = 0, enew = e_int of uold on the owned cells (godunov_fine.f90:71-90)
+    rc = launch_pfix_pass(*L, PFIX_INIT, 0.0, nullptr); if (rc) return rc;
+    L->pfix_ready = true;
+  }
   L->unew_valid = true;
   return RGPU_OK;
 }
@@ -2120,6 +2203,8 @@ int rgpu_godunov_fine_dev(int ilevel, double dt) {
   }
   Level* L; int rc = check_level(ilevel, &L); if (rc) return rc;
   if (!(dt > 0)) return fail(RGPU_EINVAL, "dt=%g", dt);
+  // pressure_fix: the sweep accumulates into divu / enew, so they must hold set_unew's values -- never a previous sweep's
+  if (G.p.pressure_fix && !L->pfix_ready) return fail(RGPU_EINVAL, "pressure_fix: rgpu_set_unew has not initialised divu / enew since the last sweep");
   // dt travels by value in the launch arguments (hydro kernels): no copy, no host synchronisation per call.  The MHD passes
   // read it from device memory: asynchronous copy from a buffer that outlives the call
   if (G.p.mhd) {
@@ -2134,6 +2219,7 @@ int rgpu_godunov_fine_dev(int ilevel, double dt) {
   L->dt_by_value = 0.0;
   if (rc) return rc;
   L->unew_valid = true;
+  L->pfix_ready = false;
   L->dt_last = dt;
   return RGPU_OK;
 }
@@ -2160,10 +2246,16 @@ int rgpu_set_uold(int ilevel) {
     CUDA_OK(cudaGetLastError());
     L->launches++;
   }
+  if (G.p.pressure_fix) {   // add_pdv_source_terms on enew from uold (godunov_fine.f90:164-168)
+    if (!(L->dt_last > 0)) return fail(RGPU_EINVAL, "set_uold with pressure_fix before godunov_fine (dtnew(ilevel) unknown)");
+    rc = launch_pfix_pass(*L, PFIX_PDV, L->dt_last, nullptr); if (rc) return rc;
+  }
   // uold <- unew on the active cells (godunov_fine.f90:193-197); shells keep their uold values
   rc = carry_shells(*L, L->d_u[L->cur], L->d_u[1 - L->cur]); if (rc) return rc;
   L->cur = 1 - L->cur;
   L->unew_valid = false;
+  L->pfix_ready = false;
+  if (G.p.pressure_fix) { rc = launch_pfix_pass(*L, PFIX_SWITCH, L->dt_last, nullptr); if (rc) return rc; }   // :203-227
   return RGPU_OK;
 }
 
@@ -2242,6 +2334,7 @@ int rgpu_godunov_fine(int ilevel, double dt, const double* uold, double* unew) {
   Level* L; int rc = check_level(ilevel, &L); if (rc) return rc;
   if (!uold || !unew) return fail(RGPU_EINVAL, "null state array");
   if (!(dt > 0)) return fail(RGPU_EINVAL, "dt=%g", dt);
+  if (G.p.pressure_fix) return fail(RGPU_EUNSUPPORTED, "pressure_fix: divu / enew live on the device; use the device-resident calls (rgpu_set_unew ... rgpu_set_uold)");
   rc = need_force(*L); if (rc) return rc;
   CUDA_OK(cudaMemcpyAsync(L->d_dt, &dt, sizeof(double), cudaMemcpyHostToDevice, G.stream));
   L->dt_last = dt;   // poisson: unew = uold + dF with the gravity predictor; the host's set_uold adds the source term
@@ -2265,6 +2358,7 @@ int rgpu_level_steps(int ilevel, int nstep, double* dt_hist, double sums_last[3]
   const bool multi = G.comm && G.nranks > 1 && !L->peers.empty();
   const bool fused = multi && L->d_emit_off != nullptr;
   const bool ovl = fused && L->overlap && G.comm_x != nullptr && !G.timing;   // per-kernel timing runs keep one sweep launch
+  const bool pfix = G.p.pressure_fix != 0;
   CUDA_OK(cudaEventRecord(G.ev2, G.stream));
   // amr_step order.  Ghost shells of uold are current on entry (upload / previous step).
   if (fused) rc = exchange_ghosts_fused(*L, L->d_u[L->cur], G.stream, G.comm); else rc = exchange_ghosts(*L, L->d_u[L->cur], false);
@@ -2282,15 +2376,27 @@ int rgpu_level_steps(int ilevel, int nstep, double* dt_hist, double sums_last[3]
       NCCL_OK(ncclAllReduce(L->d_dt, L->d_dt, 1, ncclDouble, ncclMin, G.comm, G.stream));
       if (s < nstep) CUDA_OK(cudaMemcpyAsync(L->d_hist + s, L->d_dt, sizeof(double), cudaMemcpyDeviceToDevice, G.stream));
     }
+    // pressure_fix: set_unew's divu / enew (owned cells of uold only), the sweep, then set_uold's pdV source (it reads the ghost
+    // and boundary shells of uold) and, after the swap, the energy switch.  The sweep's fused Courant partials would describe the
+    // state before the switch: dt and the sums of the next step come from a Courant scan of the switched state instead.
+    if (pfix) { rc = launch_pfix_pass(*L, PFIX_INIT, 0.0, nullptr); if (rc) return rc; }   // set_unew :333
     if (ovl) {
       // interior tiles read owned cells only: they run while the exchange of the previous step (stream s_x) fills the ghost
       // shells; the frame (outer tile ring + plane caps) waits for it.  Same kernel, same arithmetic, two launches.
       rc = launch_sweep(*L, -1, -1, 1, true); if (rc) return rc;
       CUDA_OK(cudaStreamWaitEvent(G.stream, L->ev_x, 0));
       rc = launch_sweep(*L, -1, -1, 2, true); if (rc) return rc;
-      rc = launch_reduce(*L, 2 * L->nblocks, dt_cap, L->d_hist + s + 1); if (rc) return rc;
+      if (pfix) {   // after the frame launch: the ghost shells of uold are the ones the previous step's exchange sent
+        rc = launch_pfix_pass(*L, PFIX_PDV, 0.0, L->d_dt); if (rc) return rc;
+      } else {
+        rc = launch_reduce(*L, 2 * L->nblocks, dt_cap, L->d_hist + s + 1); if (rc) return rc;
+      }
       rc = carry_shells(*L, L->d_u[L->cur], L->d_u[1 - L->cur], false); if (rc) return rc;
       L->cur = 1 - L->cur;
+      if (pfix) {   // the exchange below packs the switched state
+        rc = launch_pfix_pass(*L, PFIX_SWITCH, 0.0, L->d_dt); if (rc) return rc;
+        rc = launch_courant(*L, dt_cap, L->d_hist + s + 1); if (rc) return rc;
+      }
       CUDA_OK(cudaEventRecord(L->ev_s, G.stream));
       CUDA_OK(cudaStreamWaitEvent(G.s_x, L->ev_s, 0));
       rc = exchange_ghosts_fused(*L, L->d_u[L->cur], G.s_x, G.comm_x); if (rc) return rc;   // make_virtual_fine :505
@@ -2304,15 +2410,21 @@ int rgpu_level_steps(int ilevel, int nstep, double* dt_hist, double sums_last[3]
       continue;
     }
     rc = launch_sweep(*L, -1, -1, 0, true); if (rc) return rc;                       // set_unew + godunov_fine + set_uold  :333,:388,:423
-    rc = launch_reduce(*L, L->nblocks, dt_cap, L->d_hist + s + 1); if (rc) return rc;  // courant_fine of the next step
+    if (pfix) { rc = launch_pfix_pass(*L, PFIX_PDV, 0.0, L->d_dt); if (rc) return rc; }
+    else { rc = launch_reduce(*L, L->nblocks, dt_cap, L->d_hist + s + 1); if (rc) return rc; }  // courant_fine of the next step
     rc = carry_shells(*L, L->d_u[L->cur], L->d_u[1 - L->cur], !fused); if (rc) return rc;
     L->cur = 1 - L->cur;
+    if (pfix) {
+      rc = launch_pfix_pass(*L, PFIX_SWITCH, 0.0, L->d_dt); if (rc) return rc;
+      rc = launch_courant(*L, dt_cap, L->d_hist + s + 1); if (rc) return rc;
+    }
     if (fused) rc = exchange_ghosts_fused(*L, L->d_u[L->cur], G.stream, G.comm); else rc = exchange_ghosts(*L, L->d_u[L->cur], false);   // make_virtual_fine :505
     if (rc) return rc;
     rc = launch_boundaries(*L, L->d_u[L->cur]); if (rc) return rc;                  // make_boundary_hydro :514
   }
   if (ovl) CUDA_OK(cudaStreamWaitEvent(G.stream, L->ev_x, 0));
   L->unew_valid = false;
+  L->pfix_ready = false;
   CUDA_OK(cudaEventRecord(G.ev3, G.stream));
   if (dt_hist) CUDA_OK(cudaMemcpyAsync(dt_hist, L->d_hist, sizeof(double) * nstep, cudaMemcpyDeviceToHost, G.stream));
   double out[5];
@@ -2523,7 +2635,33 @@ int rgpu_upload_force(const double* f) {
   return RGPU_OK;
 }
 int rgpu_download_pressure_fix(double* divu, double* enew) {
-  if (!G.init || !G.amr || !G.p.pressure_fix) return fail(RGPU_EINVAL, "rgpu_download_pressure_fix needs AMR mode and rgpu_params.pressure_fix");
+  if (!G.init || !G.p.pressure_fix) return fail(RGPU_EINVAL, "rgpu_download_pressure_fix needs rgpu_params.pressure_fix");
+  if (!G.amr) {   // every bound dense level: divu / enew of its active cells; every other entry keeps the caller's value
+    const int T = T_();
+    std::vector<double> h;
+    for (int l = 1; l <= MAXLEVEL; l++) {
+      const Level& L = G.lev[l];
+      if (!L.bound || !L.dense || !L.d_pfix) continue;
+      const size_t vs = (size_t)T * L.nslot;
+      h.resize(2 * vs);
+      CUDA_OK(cudaMemcpyAsync(h.data(), L.d_pfix, sizeof(double) * 2 * vs, cudaMemcpyDeviceToHost, G.stream));
+      CUDA_OK(cudaStreamSynchronize(G.stream));
+      const DenseGeom& g = L.g;
+      for (long long s = 0; s < L.nslot; s++) {
+        const int ig = L.slot_igrid[s];
+        const int ox = (int)(s % g.nox), oy = (int)((s / g.nox) % g.noy), oz = (int)(s / ((long long)g.nox * g.noy));
+        if (ig <= 0 || 2 * ox < g.ox0 || 2 * ox >= g.ox1) continue;
+        if (G.p.ndim > 1 && (2 * oy < g.oy0 || 2 * oy >= g.oy1)) continue;
+        if (G.p.ndim > 2 && (2 * oz < g.oz0 || 2 * oz >= g.oz1)) continue;
+        for (int ind = 0; ind < T; ind++) {
+          const size_t c = (size_t)G.ncoarse + (size_t)ind * G.ngridmax + ig - 1;
+          if (divu) divu[c] = h[(size_t)ind * L.nslot + s];
+          if (enew) enew[c] = h[vs + (size_t)ind * L.nslot + s];
+        }
+      }
+    }
+    return RGPU_OK;
+  }
   if (!G.d_unew) return fail(RGPU_EINVAL, "bind the tree first");
   if (divu) CUDA_OK(cudaMemcpyAsync(divu, d_divu(), sizeof(double) * G.ncell, cudaMemcpyDeviceToHost, G.stream));
   if (enew) CUDA_OK(cudaMemcpyAsync(enew, d_enew(), sizeof(double) * G.ncell, cudaMemcpyDeviceToHost, G.stream));

@@ -75,8 +75,8 @@ struct SweepArgs {
   const double* force;
   int gsrc;                   // 1: set_uold's add_gravity_source_terms is fused into the update and the Courant scan of the
                               // new state uses sum|f| (rgpu_level_steps: f stays fixed over the steps of the call)
-  // pressure_fix (PFIX instantiation, AMR variant only): divu and enew in the level-store layout [2][2^ndim][nslot] (addressed
-  // like uout).  On entry they hold set_unew's values plus the finer level's refluxes; the sweep accumulates the face velocity
+  // pressure_fix (PFIX instantiation): divu and enew in the level-store layout [2][2^ndim][nslot] (addressed like uout).  On
+  // entry they hold set_unew's values (AMR variant: plus the finer level's refluxes); the sweep accumulates the face velocity
   // tmp1 and the internal-energy flux tmp2 into them like two more variables (hydro/godunov_fine.f90:735-745,775-786)
   double* pfix;
 };
@@ -196,8 +196,8 @@ struct SweepSmem {
   static constexpr size_t exq = HY ? (size_t)NV * NT : 0;  // qm_y
   static constexpr size_t exf = HY ? (size_t)NV * NT : 0;  // Fy
   static constexpr size_t carry = HZ ? (size_t)3 * NV * NT : 0;
-  static constexpr size_t exft = PFIX ? (size_t)2 * NT : 0;    // tmp1, tmp2 of the y faces
-  static constexpr size_t carryt = PFIX ? (size_t)4 * NT : 0;  // tmp1, tmp2 of the previous z face, partial divu / enew update
+  static constexpr size_t exft = (PFIX && HY) ? (size_t)2 * NT : 0;    // tmp1, tmp2 of the y faces
+  static constexpr size_t carryt = (PFIX && HZ) ? (size_t)4 * NT : 0;  // tmp1, tmp2 of the previous z face, partial divu / enew update
   static constexpr size_t doubles = ring + stage + fstage + exq + exf + carry + exft + carryt;
 };
 
@@ -206,14 +206,16 @@ struct SweepSmem {
 // are complete by then -- so the plane loop has two CTA barriers instead of three.  Same arithmetic in the same order.
 // GRAV (poisson): the gravity predictor with f = a.force in ctoprim of every converted cell and, when a.gsrc is set, set_uold's
 // add_gravity_source_terms in the update plus the gravity term of the fused Courant scan.
-// PFIX (pressure_fix, 3-D AMR variant): every face also yields tmp1 = half*(ql(ln)+qr(ln)) and tmp2 = the internal-energy flux of
-// the solver (hydro/umuscl.f90:844-850), scaled and masked like the fluxes; the update accumulates them into divu / enew
-// (a.pfix) in the same x, y, z order.  They travel like the fluxes: x by shuffle, y through shared memory, z in the carry.
+// PFIX (pressure_fix; the 3-D AMR variant, and the plain form without GRAV in 1-D, 2-D and 3-D): every face also yields tmp1 =
+// half*(ql(ln)+qr(ln)) and tmp2 = the internal-energy flux of the solver (hydro/umuscl.f90:844-850), scaled and masked like the
+// fluxes; the update accumulates them into divu / enew (a.pfix, initialised by set_unew) in the same x, y, z order.  They travel
+// like the fluxes: x by shuffle, y through shared memory, z in the carry.  The plain form starts the state from uin as usual.
 template <int NDIM, int RIEMANN, int SLOPE, int BX, int BY, bool AMRV = false, bool LATE = false, bool GRAV = false, bool PFIX = false>
 __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs a) {
   static_assert(!(LATE && AMRV), "the late-update variant exists for the plain dense sweep only");
   static_assert(!(LATE && GRAV), "the late-update variant exists for the plain dense sweep only");
-  static_assert(!PFIX || (AMRV && NDIM == 3), "pressure_fix exists for the 3-D AMR variant only");
+  static_assert(!PFIX || (AMRV && NDIM == 3) || (!AMRV && !GRAV), "pressure_fix: the 3-D AMR variant, or the plain form without poisson");
+  static_assert(!(LATE && PFIX), "the late-update variant exists for the plain dense sweep only");
   using S = SweepSmem<NDIM, BX, BY, GRAV, PFIX>;
   constexpr int NV = S::NV, HY = S::HY, HZ = S::HZ, QX = S::QX, QY = S::QY, NQ = S::NQ, NT = S::NT;
   constexpr int TXO = BX - 2;                 // owned cells per tile in x
@@ -533,6 +535,10 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
         } else {
 #pragma unroll
           for (int n = 0; n < NV; n++) ucur[n] = __ldg(a.uin + n * vstride + off);
+          if (PFIX) {            // set_unew's divu = 0, enew = e_int of uold
+#pragma unroll
+            for (int n = 0; n < NPF; n++) pcur[n] = a.pfix[n * vstride + off];
+          }
         }
       }
       // PFIX: tmp1 = half*(qleft(ln)+qright(ln)), tmp2 = fgdnv(nvar+1) (hydro/umuscl.f90:844-850), scaled like the fluxes (:111-112)
@@ -688,8 +694,8 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
             for (int n = 0; n < NPF; n++) {
               double p = pcur[n];
               p = p + (tx[n] - txr[n]);
-              p = p + (ty[n] - exft[n * NT + tid + BX]);
-              carryt[(2 + n) * NT + tid] = p;
+              if (HY) p = p + (ty[n] - exft[n * NT + tid + BX]);
+              if (HZ) carryt[(2 + n) * NT + tid] = p; else pnew[n] = p;
             }
           }
           if (!HZ) have = true;
@@ -765,6 +771,60 @@ __global__ void __launch_bounds__(BX * BY, 1) sweep_dense_kernel(const SweepArgs
       a.part[2 * nb + c0] = v2; a.part[3 * nb + c0] = v3;
     }
   }
+}
+
+// ---- pressure_fix passes of set_unew / set_uold on a dense level store: one thread per owned cell, divu / enew in the
+// PFIX store [2][2^ndim][nslot].  The per-cell arithmetic is the one of the AMR list kernels (hydro_device.cuh).  dt_dev != NULL:
+// the time step is read from device memory (rgpu_level_steps), otherwise dt is used.
+template <int NDIM>
+__device__ __forceinline__ bool dense_owned_cell(const DenseGeom& g, long long i, long long& off) {
+  const long long nx = g.ox1 - g.ox0, ny = NDIM > 1 ? g.oy1 - g.oy0 : 1, nz = NDIM > 2 ? g.oz1 - g.oz0 : 1;
+  if (i >= nx * ny * nz) return false;
+  const int x = g.ox0 + (int)(i % nx), y = NDIM > 1 ? g.oy0 + (int)((i / nx) % ny) : 0, z = NDIM > 2 ? g.oz0 + (int)(i / (nx * ny)) : 0;
+  off = cell_offset<NDIM>(g, x, y, z);
+  return true;
+}
+// set_unew (hydro/godunov_fine.f90:71-90): divu = 0, enew = E - e_kin of uold
+template <int NDIM>
+__global__ void dense_pfix_init_kernel(const double* __restrict__ uold, double* __restrict__ pfix, DenseGeom g, double smallr) {
+  long long off;
+  if (!dense_owned_cell<NDIM>(g, blockIdx.x * (long long)blockDim.x + threadIdx.x, off)) return;
+  const size_t vs = (size_t)(1 << NDIM) * g.nslot;
+  pfix_init_cell(uold + off, vs, pfix + off, pfix + vs + off, NDIM, smallr);
+}
+// add_pdv_source_terms (:294-437): enew -= (gamma-1) e_old div(u) dt from the face neighbours in uold.  On a full level every face
+// neighbour of an owned cell is a cell of the box at distance dx -- owned, a ghost or boundary oct of the shell, or the periodic
+// image -- so the reference's fallback to the father cell at 1.5 dx never applies (rgpu_bind_level refuses a shell with a hole)
+template <int NDIM>
+__global__ void dense_pdv_kernel(const double* __restrict__ uold, double* __restrict__ pfix, DenseGeom g, double gamma, double smallr,
+                                 double dx, double dt, const double* __restrict__ dt_dev) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  long long off;
+  if (!dense_owned_cell<NDIM>(g, i, off)) return;
+  const long long nx = g.ox1 - g.ox0, ny = NDIM > 1 ? g.oy1 - g.oy0 : 1;
+  const int c[3] = {g.ox0 + (int)(i % nx), NDIM > 1 ? g.oy0 + (int)((i / nx) % ny) : 0, NDIM > 2 ? g.oz0 + (int)(i / (nx * ny)) : 0};
+  const int n[3] = {g.ncx, g.ncy, g.ncz}, w[3] = {g.wrapx, g.wrapy, g.wrapz};
+  const size_t vs = (size_t)(1 << NDIM) * g.nslot;
+  auto uo = [&](long long o, int k) -> double { return uold[k * vs + o]; };
+  double divu_loc = 0.0;
+#pragma unroll
+  for (int d = 0; d < NDIM; d++) {
+    int l[3] = {c[0], c[1], c[2]}, r[3] = {c[0], c[1], c[2]};
+    l[d] = wrap_or_clamp(c[d] - 1, n[d], w[d]);
+    r[d] = wrap_or_clamp(c[d] + 1, n[d], w[d]);
+    const long long ol = cell_offset<NDIM>(g, l[0], l[1], l[2]), orr = cell_offset<NDIM>(g, r[0], r[1], r[2]);
+    divu_loc = pdv_face_term(divu_loc, uo, ol, orr, d, dx, dx, smallr);
+  }
+  pfix[vs + off] = pdv_cell(pfix[vs + off], divu_loc, uo, off, NDIM, gamma, smallr, dt_dev ? *dt_dev : dt);
+}
+// set_uold's energy switch (:203-227) on the new state, in place
+template <int NDIM>
+__global__ void dense_pfix_switch_kernel(double* __restrict__ uold, const double* __restrict__ pfix, DenseGeom g, double smallr,
+                                         double beta_fix, double dx, double dt, const double* __restrict__ dt_dev) {
+  long long off;
+  if (!dense_owned_cell<NDIM>(g, blockIdx.x * (long long)blockDim.x + threadIdx.x, off)) return;
+  const size_t vs = (size_t)(1 << NDIM) * g.nslot;
+  pfix_switch_cell(uold + off, vs, pfix + off, pfix + vs + off, NDIM, smallr, beta_fix, dx, dt_dev ? *dt_dev : dt);
 }
 
 // tile shapes (a warp = one x-row of 32 cells): BX = 32, BY = tile height in rows (threads = 32*BY).
@@ -843,6 +903,22 @@ cudaError_t launch_sweep_dense_pfix(const SweepArgs& a, int nblocks, cudaStream_
   constexpr int BX = 32, BY = tile_by_default(3, RIEMANN);
   constexpr size_t smem = sizeof(double) * SweepSmem<3, BX, BY, GRAV, true>::doubles;
   auto kern = sweep_dense_kernel<3, RIEMANN, -1, BX, BY, true, false, GRAV, true>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    configured = true;
+  }
+  kern<<<nblocks, dim3(BX, BY, 1), smem, st>>>(a);
+  return cudaGetLastError();
+}
+// pressure_fix (PFIX) outside AMR mode: the plain form without poisson, one instantiation per dimension and solver with the
+// runtime slope switch and the default tile height (sweep_pfix_inst_plain_*.cu)
+template <int NDIM, int RIEMANN>
+cudaError_t launch_sweep_dense_pfix_plain(const SweepArgs& a, int nblocks, cudaStream_t st) {
+  constexpr int BX = 32, BY = tile_by_default(NDIM, RIEMANN);
+  constexpr size_t smem = sizeof(double) * SweepSmem<NDIM, BX, BY, false, true>::doubles;
+  auto kern = sweep_dense_kernel<NDIM, RIEMANN, -1, BX, BY, false, false, false, true>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
